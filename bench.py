@@ -1,9 +1,10 @@
-"""bench.py -- MoCo pretrain images/sec on N B200s (BASELINE.json metric), plus the kernel roofline.
+"""bench.py -- MoCo pretrain images/sec on N H100s (BASELINE.json metric), plus the kernel roofline.
 
     python bench.py --gpus 1 --steps 20 --warmup 5
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference ...      # CPU arm: the UNMODIFIED reference train_moco (oracle/_ref) on host cores
+    python bench.py ... --dump-outputs DIR    # also write what the timed path computed in its last step (DIR/<name>.npy)
 
 A step = one MoCo iteration (train.py:244-283): query encoder fwd, ShuffleBN permute, key encoder fwd,
 un-shuffle, q.Queue^T + InfoNCE + dq, enqueue, backward, SGD step, EMA update -- ResNet-50, feat_dim 128,
@@ -52,16 +53,11 @@ def parse():
     ap.add_argument("--no-sharded", action="store_true", help="N>1: skip the configs[3] sharded-queue block")
     ap.add_argument("--ddp-bucket-mb", type=int, default=25)
     ap.add_argument("--ddp-bf16", action="store_true", help="N>1: all-reduce gradients as bf16 (DDP compress hook)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write rank 0's outputs of the last timed step (loss, prob, queue, ring "
+                         "index, a seeded sample of both encoders' parameters) as DIR/<name>.npy, float32 / float64, "
+                         "at most 64 MB in all")
     return ap.parse_args()
-
-
-# dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel, from the committed `ncu --set full`
-# captures of this round (profiles/r2_*_ncu_metrics.csv; tools/gpu_lab.py op_c2 / op_c3 / op_c5 under ncu)
-NCU_TRAFFIC_BYTES = {
-    ("onepass", 256, 128, 16384): 4332544,                       # profiles/r2_head128_c2_ncu_metrics.csv
-    ("onepass", 256, 128, 65536): 16915200,                      # profiles/r2_head128_c3_ncu_metrics.csv (0 B written: L2)
-    ("onepass", 512, 256, 262144): 134541312 + 3316992,          # profiles/r2_head256_c5_ncu_metrics.csv
-}
 
 
 def load_peaks():
@@ -69,8 +65,10 @@ def load_peaks():
     if os.path.exists(path):
         d = json.load(open(path))
         return {"hbm_gbs": d["hbm_gbs"], "tf_burst": d["bf16_tflops"], "tf_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
-                "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "tf_burst": 1590.0, "tf_sustained": 1400.0, "source": "fallback (B200_PROFILING.md)"}
+                "source": "measured (MEASURED_PEAKS.json)", "tf_kind": "sustained bf16"}
+    # NVIDIA's H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 dense bf16 TFLOP/s -- nominal, not reached figures
+    return {"hbm_gbs": 3350.0, "tf_burst": 989.0, "tf_sustained": 989.0, "source": "H100 SXM data sheet",
+            "tf_kind": "nominal dense bf16 (700 W card)"}
 
 
 class ClockSampler(threading.Thread):
@@ -177,6 +175,47 @@ def run_reference(args):
     print(json.dumps(line))
 
 
+def sm_count(dev):
+    import torch
+    return torch.cuda.get_device_properties(dev).multi_processor_count
+
+
+DUMP_MAX_BYTES = 64 << 20
+
+
+def write_outputs(out_dir, arrays):
+    """arrays: name -> tensor / ndarray; each is written as out_dir/<name>.npy (float64 stays, the rest float32).
+    At most DUMP_MAX_BYTES in all."""
+    import numpy as np
+    import torch
+    out = {}
+    for name, a in arrays.items():
+        if isinstance(a, torch.Tensor):
+            a = a.detach().cpu().numpy()
+        a = np.asarray(a)
+        out[name] = a if a.dtype == np.float64 else a.astype(np.float32)
+    total = sum(a.nbytes for a in out.values())
+    if total > DUMP_MAX_BYTES:
+        raise RuntimeError(f"--dump-outputs: {total} bytes exceed the {DUMP_MAX_BYTES}-byte limit")
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in out.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
+def flat_sample(flat, n, seed=0):
+    """A fixed, seeded sample of n elements of the 1-D tensor `flat` (in index order)."""
+    import torch
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    idx = torch.randperm(flat.numel(), generator=g)[: min(n, flat.numel())].sort().values
+    return flat[idx.to(flat.device)]
+
+
+def param_sample(module, n=1 << 20, seed=0):
+    """A fixed, seeded sample of n elements of all parameters of `module` (flattened in parameters() order)."""
+    import torch
+    return flat_sample(torch.cat([p.detach().reshape(-1).float() for p in module.parameters()]), n, seed)
+
+
 def stress_roofline(peaks, dev):
     """BASELINE configs[4]: N=512, C=256, K=262144 -- the tensor-bound shape, hot-path kernels alone (queue 134 MB > L2).
     Default path = ONE sweep over the queue producing loss statistics AND dq (4NCK FLOP); the two-pass alternative
@@ -222,19 +261,18 @@ def stress_roofline(peaks, dev):
 
     _, us_one = timed_kernels(_lib.NCE_AUTO)                      # one-pass kernel reports on the DQ hook
     win = ctypes.c_float()
-    lib.moco_prof_sweep_window(wp, 148, ctypes.byref(win), stream)
+    lib.moco_prof_sweep_window(wp, sm_count(dev), ctypes.byref(win), stream)
     us_stats, us_dq = timed_kernels(_lib.NCE_TWO_PASS)
     flops = 2.0 * N * C * (K + 1)                                 # per direction (SURVEY.md 8d): fwd = bwd = 2NC(K+1)
     bytes_ = K * C * 2 + 3 * N * C * 2 + 12 * N
     a = 2 * flops / (us_one * 1e-6) / 1e12
     return {
         "workload": "BASELINE configs[4]: N=512 feat_dim=256 K=262144 (hot-path kernels alone, queue 134 MB > L2)",
-        "kernel": "nce_head256_kernel<FUSED> (one sweep on tcgen05: S=q.Queue^T, P=2^(S/T-m), O+=P.Queue, row sums; q half in "
-                  "TMEM / half in smem, three S buffers) -> loss statistics + dq partials; the tail kernel finishes both",
+        "kernel": "nce_sweep_kernel<4, kFused> (one sweep on wgmma: S=q.Queue^T, P=2^(S/T-m) in registers, O+=P.Queue, "
+                  "row sums) -> loss statistics + dq partials; the tail kernel finishes both",
         "bound": "tensor", "achieved": a, "peak": peaks["tf_burst"], "unit": "TFLOP/s", "frac": a / peaks["tf_burst"],
         "us_per_launch": us_one, "device_window_us": float(win.value),
         "algorithmic_flops": 2 * flops, "hbm_GBps": bytes_ / (us_one * 1e-6) / 1e9,
-        "traffic": NCU_TRAFFIC_BYTES.get(("onepass", N, C, K)),
         "two_pass": {"stats_kernel_us": us_stats, "stats_TFLOPs": flops / (us_stats * 1e-6) / 1e12,
                      "stats_frac": flops / (us_stats * 1e-6) / 1e12 / peaks["tf_burst"],
                      "dq_kernel_us": us_dq, "dq_TFLOPs_executed": 2 * flops / (us_dq * 1e-6) / 1e12,
@@ -291,7 +329,7 @@ def shufflebn_block(x2, epoch, rank, world, dev, nhwc):
             "row_layout": "bf16 NHWC [224, 224, 3]" if nhwc else "bf16 NCHW",
             "gather_GBps": n * row_bytes / (gather_us * 1e-6) / 1e9,
             "nvlink_GBps": remote * row_bytes / (gather_us * 1e-6) / 1e9,
-            "nvlink_frac_of_900": remote * row_bytes / (gather_us * 1e-6) / 1e9 / 900.0,
+            "nvlink_frac_of_450": remote * row_bytes / (gather_us * 1e-6) / 1e9 / 450.0,   # NVLink 4: 450 GB/s per direction
             "note": "fwd_us = publish (crop+cast+layout into the peer-mapped staging buffer) + signal barrier + pull; "
                     "gather_us = the pull kernel alone; nvlink_GBps counts only rows that live on another GPU "
                     "(this rank's count; slowest rank's time)"}
@@ -374,7 +412,11 @@ def run_native(args):
         dist.init_process_group("nccl", device_id=dev)
     lib = _lib.load()
     peaks = load_peaks()
-    torch.backends.cudnn.benchmark = True
+    # fixed, deterministic cuDNN algorithms: autotuning (cudnn.benchmark) chooses convolution kernels by timing, which
+    # varies from run to run, and several of them accumulate with atomics -- either way two runs with the same
+    # arguments would train on different roundings and --dump-outputs could not compare builds output for output
+    torch.backends.cudnn.benchmark = False
+    torch.backends.cudnn.deterministic = True
     torch.backends.cuda.matmul.allow_tf32 = True
     torch.backends.cudnn.allow_tf32 = True
 
@@ -446,19 +488,21 @@ def run_native(args):
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         return float(ms)
 
-    # ---- arm 1: inputs resident in HBM (308 MB per step > 126 MB L2)
+    # ---- arm 1: inputs resident in HBM (308 MB per step > 50 MB L2)
     x1, x2 = split(dev_inputs)
     ev = [[torch.cuda.Event(enable_timing=True) for _ in range(4)] for _ in range(args.steps)]
     for e4 in ev:
         for j in (1, 0, 3, 2):       # stop before start: a hook that never fires reads as a negative interval
             e4[j].record()
 
+    last = {}
+
     def loop_resident(steps, profile=False):
         for i in range(steps):
             if profile:
                 lib.moco_prof_set_events(1, ev[i][0].cuda_event, ev[i][1].cuda_event)
                 lib.moco_prof_set_events(2, ev[i][2].cuda_event, ev[i][3].cuda_event)
-            step(x1, x2, epoch)
+            last["loss"], last["prob"] = step(x1, x2, epoch)
 
     loop_resident(args.warmup)
     sampler = ClockSampler(local_rank)
@@ -470,9 +514,20 @@ def run_native(args):
     sampler.join()
     lib.moco_prof_set_events(1, None, None)
     lib.moco_prof_set_events(2, None, None)
+    if args.dump_outputs and rank == 0:
+        # the last timed step's results, before anything below runs more steps (same seeds -> same inputs every run).
+        # Rank 0 only: the queue is replicated and DDP keeps the parameters identical on every rank.  A queue above
+        # 32 MB (K * C > 8M) is written as a seeded sample of 8M elements.
+        enc = model.module if world > 1 else model
+        q_flat, q_max = contrast.memory.reshape(-1), 8 << 20
+        queue = {"queue": contrast.memory} if q_flat.numel() <= q_max else {"queue_sample": flat_sample(q_flat, q_max)}
+        write_outputs(args.dump_outputs, {
+            "loss": last["loss"].reshape(1), "prob": last["prob"].reshape(1), **queue,
+            "queue_index": torch.tensor([float(contrast.index)], dtype=torch.float64),
+            "encoder_q_params_sample": param_sample(enc), "encoder_k_params_sample": param_sample(model_ema)})
     win = ctypes.c_float()
     sc = next(iter(contrast._scratch.values()))
-    lib.moco_prof_sweep_window(sc.ws_ptr, 148, ctypes.byref(win), torch.cuda.current_stream().cuda_stream)
+    lib.moco_prof_sweep_window(sc.ws_ptr, sm_count(dev), ctypes.byref(win), torch.cuda.current_stream().cuda_stream)
     us_stats = sum(e[0].elapsed_time(e[1]) for e in ev) * 1e3 / args.steps
     us_dq = sum(e[2].elapsed_time(e[3]) for e in ev) * 1e3 / args.steps
     ms_step = ms_total / args.steps
@@ -540,7 +595,7 @@ def run_native(args):
                                 "steps; bytes = 2 B x elements x (statistics 1 + apply 2 [+1 residual]) forward, "
                                 "(reduce 2 [+1 mask] + apply 3 [+1 mask] [+1 d residual]) backward"},
             "note": "ATen arm = nn.BatchNorm2d's own bf16 channels_last kernels + separate add and ReLU passes, everything "
-                    "else identical (same MoCoStep, same head kernels); profiles/ has the per-kernel ncu captures"}
+                    "else identical (same MoCoStep, same head kernels)"}
 
     shufflebn = sharded = None
     if world > 1:
@@ -575,20 +630,19 @@ def run_native(args):
     us_main = us_dq if one_pass else us_stats + us_dq
     a_tf = flops / (us_main * 1e-6) / 1e12
     roofline = {
-        "kernel": ("nce_head128_kernel<FUSED>: one sweep over the queue on tcgen05 (q staged in-kernel, S = q.Queue^T, "
+        "kernel": ("nce_sweep_kernel<2, kFused>: one sweep over the queue on wgmma (q staged in-kernel, S = q.Queue^T, "
                    "P = 2^(S/T - m), O += P.Queue, row sums) -> loss statistics + dq partials" if one_pass else
-                   "nce_stats_kernel + nce_head128_kernel (two-pass)") + ", timed inside the step",
+                   "nce_sweep_kernel<2, kStats> + nce_sweep_kernel<2, kNormed> (two-pass)") + ", timed inside the step",
         "bound": "tensor", "achieved": a_tf, "peak": peaks["tf_sustained"], "unit": "TFLOP/s",
-        "frac": a_tf / peaks["tf_sustained"], "peak_source": peaks["source"] + ", sustained bf16",
+        "frac": a_tf / peaks["tf_sustained"], "peak_source": peaks["source"] + ", " + peaks["tf_kind"],
         "us_per_launch": us_main, "algorithmic_flops": flops, "algorithmic_bytes": bytes_,
         "device_window_us": float(win.value),
         "device_window_note": "first CTA entry -> last CTA exit of the last sweep kernel on the device clock (%globaltimer): "
                               "what the CTAs took; us_per_launch (CUDA events around the single kernel, which breaks its "
-                              "programmatic-dependent-launch overlap) also contains ~4.5 us of grid launch and ~2 us of completion",
+                              "programmatic-dependent-launch overlap) also contains the grid launch and completion latency",
         "hbm_GBps": bytes_ / (us_main * 1e-6) / 1e9, "hbm_frac": bytes_ / (us_main * 1e-6) / 1e9 / peaks["hbm_gbs"],
-        "traffic": NCU_TRAFFIC_BYTES.get(("onepass", N, C, K)),
         "note": f"ideal time for this shape is {flops / (peaks['tf_sustained'] * 1e12) * 1e6:.1f} us "
-                f"({flops / 1e9:.2f} GFLOP, {bytes_ / 1e6:.1f} MB): {-(-K // 128 * ((N + 127) // 128) // 148)} 128-row tile(s) per CTA, "
+                f"({flops / 1e9:.2f} GFLOP, {bytes_ / 1e6:.1f} MB): {-(-K // 128 * ((N + 127) // 128) // sm_count(dev))} 128-row tile(s) per CTA, "
                 "so launch + prologue + one pipeline fill + the split-K partials dominate; roofline_stress (N=1 runs) is "
                 "the tensor-bound shape of BASELINE configs[4]",
     }
@@ -597,6 +651,7 @@ def run_native(args):
         "n_gpus": world, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_step,
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "bf16", "data": "synthetic",
         "config": config_block(args, K, world),
+        "cudnn": "fixed deterministic algorithms (cudnn.benchmark off, cudnn.deterministic on)",
         "clocks": sampler.result(),
         "e2e": {"value": e2e_value, "unit": "images/s", "ms_per_step": ms_e2e / args.steps,
                 "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 8},
@@ -619,8 +674,11 @@ def run_native(args):
     if world == 1 and not args.no_stress:
         line["roofline_stress"] = stress_roofline(peaks, dev)
     if world == 1 and not args.no_cpu_baseline:
-        r = reference_job(args.arch, C, K, T, args.cpu_sample_batch, 5, 3)
-        line["cpu_baseline"] = cpu_baseline_block(r)
+        if os.path.isfile(os.path.join(ROOT, "oracle", "_ref", "train.py")):
+            r = reference_job(args.arch, C, K, T, args.cpu_sample_batch, 5, 3)
+            line["cpu_baseline"] = cpu_baseline_block(r)
+        else:       # the reference is staged by __graft_entry__.build() only where its checkout exists
+            line["cpu_baseline"] = {"value": None, "note": "not run: oracle/_ref (the staged reference) is absent"}
     print(json.dumps(line))
     if world > 1:
         dist.barrier()

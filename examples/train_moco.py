@@ -1,4 +1,4 @@
-"""Minimal MoCo pre-training driver on the B200-native hot path -- what bl0/moco's ``train.py`` main loop
+"""Minimal MoCo pre-training driver on the H100-native hot path -- what bl0/moco's ``train.py`` main loop
 (train.py:231-293) looks like once ``MemoryMoCo`` / ``DistributedShufle`` / ``moment_update`` come from
 ``moco_b200`` (INTEGRATION.md).  Not a port of the reference's control plane (logging, LR schedule, dataset,
 checkpoint rotation are out of scope, SURVEY.md §8): synthetic images, SGD, N steps.

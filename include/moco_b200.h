@@ -1,5 +1,5 @@
 /*
- * moco_b200 -- C ABI of the B200-native MoCo contrastive hot path.
+ * moco_b200 -- C ABI of the H100-native MoCo contrastive hot path.
  *
  * This is the drop-in boundary (SURVEY.md §8b).  The reference (bl0/moco) is pure
  * Python on PyTorch and has no FFI of its own; each entry point below replaces
@@ -39,14 +39,13 @@ enum {
 
 enum { MOCO_F32 = 0, MOCO_BF16 = 1 };
 
-/* moco_nce_fwd `flags` (0 = the tuned defaults).  ABI 2 removed the round-1 variants that measured slower or
- * time-neutral (TMA-multicast sharing, first-generation dq kernel, q-in-TMEM statistics kernel, 8-warp epilogue,
- * one-chunk CTA-pair stages); their bit values (8, 16, 32, 64, 128, 256) stay reserved. */
+/* moco_nce_fwd `flags` (0 = the tuned defaults).  Bit values 8, 16, 32, 64, 128 and 256 belonged to removed
+ * kernel variants and stay reserved. */
 enum {
-    MOCO_NCE_AUTO = 0,         /* tcgen05 kernels when the shape allows it (C % 64 == 0, C <= 256)   */
+    MOCO_NCE_AUTO = 0,         /* wgmma kernels when the shape allows it (C % 64 == 0, C <= 256)     */
     MOCO_NCE_FORCE_SIMT = 1,   /* generic CUDA-core kernel (any shape)                               */
-    MOCO_NCE_CTA_PAIR = 2,     /* statistics kernel on tcgen05.mma.cta_group::2 (M = 256 per pair)   */
-    MOCO_NCE_SINGLE_CTA = 4,   /* require the tcgen05 path (error instead of the generic fallback)   */
+    MOCO_NCE_CTA_PAIR = 2,     /* statistics kernel on 2-CTA clusters sharing each queue tile (TMA multicast) */
+    MOCO_NCE_SINGLE_CTA = 4,   /* require the tensor-core path (error instead of the generic fallback) */
     MOCO_NCE_TWO_PASS = 512,   /* statistics pass, then dq pass normalised with the final lse (always exact) */
     MOCO_NCE_ONE_PASS = 1024   /* loss AND dq from one sweep over the queue (4NCK FLOP, NK exps instead of   */
                                /* 6NCK, 2NK) plus ONE tail kernel: each (CTA, row) stabilises with the row   */
@@ -85,7 +84,7 @@ int moco_device_info(int* sm_count, int* cc_major, int* cc_minor);
  * PRE-enqueue snapshot (Contrast.py:25) -- call moco_queue_enqueue afterwards on
  * the same stream.  Because dq is produced here, before the enqueue, no clone of
  * the queue is ever needed (the reference clones it every step, Contrast.py:24-25).
- * The contractions run on tcgen05 tensor cores with bf16 operands (q is rounded
+ * The contractions run on wgmma tensor cores with bf16 operands (q is rounded
  * to bf16 when given as f32) and fp32 accumulation; the positive logit is
  * computed in fp32 from the inputs as given.
  * `logits` ([N, K+1] fp32, row stride K+1) may be NULL: then no logit ever
@@ -107,7 +106,7 @@ int moco_nce_fwd(const void* q, const void* k, int qk_dtype,
  * (moco/NCE/Contrast.py:20-36) + NCESoftmaxLoss (NCECriterion.py:11-13) + `prob`
  * (train.py:264) + the gradient of train.py:273:
  *
- *   kernel 1  the q.Queue^T sweep on tcgen05 (reads q as given, no cast kernel);
+ *   kernel 1  the q.Queue^T sweep on wgmma (reads q as given, no cast kernel);
  *   kernel 2  merge -> lse / loss / prob, weighted sum of the partial gradients -> dq,
  *             then queue[(index + i) mod K] = k_all[i] for i in [0, n_all), and the
  *             ring position advanced on the device when `index_dev` is given.
@@ -140,7 +139,7 @@ enum { MOCO_PROF_STATS = 1, MOCO_PROF_DQ = 2 };   /* one-pass mode: its single k
 int moco_prof_set_events(int kernel, void* ev_start, void* ev_stop);
 /* Device-clock window of the LAST sweep kernel that ran on `workspace` (first CTA entry -> last CTA exit, %globaltimer,
  * microseconds): what the kernel's CTAs took, without the grid-launch and completion latency a CUDA-event pair around
- * a single kernel also contains.  Synchronises `stream`.  n_ctas: upper bound on the grid (148 on B200). */
+ * a single kernel also contains.  Synchronises `stream`.  n_ctas: upper bound on the grid (the SM count). */
 int moco_prof_sweep_window(const void* workspace, int n_ctas, float* us_out, void* stream);
 /* Backward of the dense-logits compatibility API (MemoryMoCo.forward returning
  * `out`, then an arbitrary upstream gradient):

@@ -2,12 +2,12 @@
 
 Mirrors ``moco/NCE/Contrast.py:6-36`` of bl0/moco (same constructor, attributes,
 buffers, ``state_dict`` keys and ``forward(q, k, k_all) -> [N, K+1]`` contract) but
-every device-side step is a hand-written sm_100a kernel reached through the C ABI
+every device-side step is a hand-written sm_90a kernel reached through the C ABI
 (``include/moco_b200.h``):
 
 * ``forward_loss(q, k, k_all) -> (loss, prob)``: the fused fast path.  The
   q.Queue^T contraction, /T, log-sum-exp, cross-entropy, ``prob`` metric AND the
-  gradient w.r.t. q are produced by tcgen05 kernels before the enqueue; the
+  gradient w.r.t. q are produced by tensor-core (wgmma) kernels before the enqueue; the
   [N, K+1] logits never reach HBM and the queue is never cloned.
 * ``forward(q, k, k_all) -> out``: API-compatible dense logits (the kernel's
   epilogue writes them).  The returned tensor also carries the fused loss so that

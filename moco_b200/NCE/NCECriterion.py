@@ -2,7 +2,7 @@
 
 ``forward(x)`` is CrossEntropyLoss(x, label 0) with mean reduction.  When ``x`` is
 the tensor ``moco_b200.NCE.MemoryMoCo.forward`` just returned (unmodified), the
-loss was already produced by the fused tcgen05 kernel (with its own backward to
+loss was already produced by the fused tensor-core kernel (with its own backward to
 q), so it is returned as is and the [N, K+1] logits are not read again.  For any
 other input the definition is evaluated directly.
 """

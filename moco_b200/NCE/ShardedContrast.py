@@ -2,7 +2,7 @@
 
 Same math as ``moco/NCE/Contrast.py`` (bl0/moco) for a queue of K rows, but rank r stores only ring
 slots [r*K/W, (r+1)*K/W): 1/W of the memory and of the HBM bytes per step.  Every rank scores ALL W*N
-queries of the step against its shard on the tcgen05 kernels (one sweep); three small exchanges stitch
+queries of the step against its shard on the tensor-core kernels (one sweep); three small exchanges stitch
 the softmax together -- the step's queries, one (max, sum) pair per query and shard, and the [W*N, C]
 partial gradients.  None of them is an NCCL collective: each rank PUBLISHES into a peer-mapped staging
 buffer (the kernels write their outputs straight into it), a stream-ordered signal barrier follows, and

@@ -1,6 +1,6 @@
 """ctypes binding of libmoco_b200.so (the C ABI in include/moco_b200.h).
 
-The library is built in-tree by ``moco_b200/build.py`` (nvcc, sm_100a).  There is
+The library is built in-tree by ``moco_b200/build.py`` (nvcc, sm_90a).  There is
 no CPU fallback: if the shared object is missing and cannot be built, importing
 any compute entry point raises.
 """

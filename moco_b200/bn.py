@@ -2,8 +2,7 @@
 
 The reference's encoders apply ``nn.BatchNorm2d`` -> [``out += residual``] -> [``nn.ReLU``] at
 ``moco/models/resnet.py:42-63,74-102,114,139-143,156-157``; ShuffleBN (``moco/util.py:69-93``) exists for exactly these
-batch statistics.  Left to ATen's channels_last kernels they are 64 % of the GPU time of a step
-(``profiles/r2_bench_launches_by_kernel.csv``).  :class:`BatchNormAct2d` is an ``nn.BatchNorm2d`` (same parameters,
+batch statistics, and left to ATen's channels_last kernels they take most of the GPU time of a step.  :class:`BatchNormAct2d` is an ``nn.BatchNorm2d`` (same parameters,
 buffers and ``state_dict`` keys, same running-statistics updates) whose training-mode forward / backward on CUDA
 bf16 channels_last activations are two launches each of ``csrc/bn_nhwc.cu`` (``moco_bn_fwd_train`` / ``moco_bn_bwd``).
 Everything else -- CPU tensors, eval mode, fp32 or NCHW activations, channel counts the kernels do not take -- runs

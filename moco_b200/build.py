@@ -1,4 +1,4 @@
-"""Build libmoco_b200.so in-tree with nvcc for sm_100a (no torch extension machinery:
+"""Build libmoco_b200.so in-tree with nvcc for sm_90a (no torch extension machinery:
 the library is plain C ABI, loaded with ctypes)."""
 import os
 import subprocess
@@ -7,11 +7,11 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libmoco_b200.so")
-SOURCES = ["capi.cu", "nce_support.cu", "nce_tail.cu", "nce_sm100.cu", "nce_head128_sm100.cu", "nce_head256_sm100.cu",
-           "queue_shuffle.cu", "ema.cu", "bn_nhwc.cu", "pool_nhwc.cu"]
-HEADERS = ["common.cuh", "sm100_ptx.cuh", "tc_common.cuh", "nce_rows.cuh", os.path.join("..", "..", "include", "moco_b200.h")]
+SOURCES = ["capi.cu", "nce_support.cu", "nce_tail.cu", "nce_sweep_sm90.cu", "queue_shuffle.cu", "ema.cu", "bn_nhwc.cu",
+           "pool_nhwc.cu"]
+HEADERS = ["common.cuh", "sm90_ptx.cuh", "tc_common.cuh", "nce_rows.cuh", os.path.join("..", "..", "include", "moco_b200.h")]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared", "-cudart", "shared",
 ]
 
@@ -40,18 +40,6 @@ def build(force=False, verbose=False):
     if verbose:
         sys.stderr.write(res.stdout + res.stderr)
     return LIB
-
-
-def build_trace_variant():
-    """Lab-only: the same sources with -DMOCO_TRACE (kernel timeline stamps) as libmoco_b200_trace.so."""
-    out = os.path.join(HERE, "libmoco_b200_trace.so")
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    cmd = [nvcc] + NVCC_FLAGS + ["-DMOCO_TRACE"] + [os.path.join(CSRC, s) for s in SOURCES] + ["-o", out]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    if res.returncode != 0:
-        sys.stderr.write(res.stdout + res.stderr)
-        raise RuntimeError("nvcc failed building the trace variant")
-    return out
 
 
 if __name__ == "__main__":

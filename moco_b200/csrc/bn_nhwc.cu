@@ -1,8 +1,7 @@
 // Training-mode batch normalisation of channels_last (NHWC) bf16 activations with the ReLU and the residual add of the
 // ResNet blocks folded in: the consumer of ShuffleBN's output (ShuffleBN exists so that these batch statistics cannot
-// leak the positive pair) and, measured, 64 % of the GPU time of a MoCo step when left to ATen's kernels
-// (profiles/r2_bench_launches_by_kernel.csv: batch_norm_collect_statistics_channels_last 30 %, transform_input 18 %,
-// backward_reduce 11 %, backward_elemt 5 %, + the separate ReLU and add passes).
+// leak the positive pair) and most of the GPU time of a MoCo step when left to ATen's kernels (statistics, transform,
+// backward reduce / element-wise, + the separate ReLU and add passes).
 //
 // Reference call sites: moco/models/resnet.py:42-63 (BasicBlock), :74-102 (Bottleneck: bn -> relu, bn -> relu,
 // bn -> += residual -> relu), :114,156-157 (stem), :139-143 (downsample conv -> bn).  Semantics = torch.nn.BatchNorm2d
@@ -39,14 +38,12 @@ constexpr int kBnRows = kBnThreads / kBnLanes;       // rows per pass
 constexpr int kBnMaxSlabs = 32;                      // C <= 2048
 constexpr int kBnPartial = 2 * kBnSlab;              // floats per CTA partial
 // (16-byte loads in flight per thread and operand, resident CTAs per SM) of each kernel; every grid is one resident
-// wave.  Measured over the 53 layers of ResNet-50 at batch 256 (tools/bn_kernel_times.py, us per encoder pass):
-//   statistics  (4,4) 1652  (8,3) 1748  (8,2) 1610  (2,4) 1773      apply      (4,3) 2527  (4,4) 2372  (8,2) 2145  (2,4) 2531
-//   bwd reduce  (4,2) 2809  (4,3) 4586  (2,4) 3689  (2,3) 3294      bwd apply  (4,2) 4818  (4,3) 6816  (2,4) 5342  (2,3) 4601
+// wave (tools/bn_kernel_times.py times the variants over the layers of ResNet-50).
 constexpr int kBnStatsUnroll = 8, kBnStatsCtas = 2;
 constexpr int kBnApplyUnroll = 8, kBnApplyCtas = 2;
 constexpr int kBnBwdReduceUnroll = 4, kBnBwdReduceCtas = 2;
 constexpr int kBnBwdApplyUnroll = 2, kBnBwdApplyCtas = 3;
-constexpr int kBnSms = 148;
+constexpr int kBnSms = 132;
 constexpr int kBnMaxCtas = kBnSms * 4;               // workspace sizing: no reduction grid is larger
 
 __device__ __forceinline__ void unpack8(const uint4& u, float* f) {

@@ -76,16 +76,17 @@ size_t moco_nce_workspace_bytes(int N, int C, int K) {
 
 }  // extern "C"
 
-// The q.Queue^T sweep (one-sweep mode when lse == nullptr): C in {64, 128} on nce_head128_sm100.cu, which reads q as
-// given (fp32/bf16, optional L2 normalisation); C in {192, 256} on nce_dq2_sm100.cu, which needs the bf16 copy `qb`.
+// The q.Queue^T sweep (one-sweep mode when lse == nullptr, nce_sweep_sm90.cu): C in {64, 128} reads q as given
+// (fp32/bf16, optional L2 normalisation); C in {192, 256} reads the bf16 copy `qb` (a 16-byte piece of an fp32 row
+// per thread would not keep a row inside one warp for the norm).
 static cudaError_t launch_sweep(const void* q, int q_dtype, int normalize, const __nv_bfloat16* qb,
                                 const __nv_bfloat16* queue, int N, int C, int K, float inv_T, const float* lse, int sms,
                                 int* slices, int* n_pad, const NceWorkspace& ws, cudaStream_t stream,
                                 bool plan_only = false) {
     if (C == 64 || C == 128)
-        return launch_nce_head128(q, q_dtype, normalize, queue, N, C, K, inv_T, lse, sms, slices, n_pad, ws, stream, plan_only);
+        return launch_nce_sweep(q, q_dtype, normalize, queue, N, C, K, inv_T, lse, sms, slices, n_pad, ws, stream, plan_only);
     if (normalize) return cudaErrorNotSupported;
-    return launch_nce_dq2_tc(qb, queue, N, C, K, inv_T, lse, sms, slices, n_pad, ws, stream, plan_only);
+    return launch_nce_sweep(qb, MOCO_BF16, 0, queue, N, C, K, inv_T, lse, sms, slices, n_pad, ws, stream, plan_only);
 }
 
 struct EnqueueSpec {            // n_all == 0: no enqueue
@@ -121,14 +122,14 @@ static int nce_head(const void* q, const void* k, int qk_dtype, int normalize, c
     const bool aligned = ((reinterpret_cast<uintptr_t>(q) & 15) == 0) && ((reinterpret_cast<uintptr_t>(queue) & 15) == 0);
     const bool tc_shape = (C % 64 == 0) && C <= 256 && aligned;
     const bool want_tc = !(flags & MOCO_NCE_FORCE_SIMT);
-    if ((flags & (MOCO_NCE_CTA_PAIR | MOCO_NCE_SINGLE_CTA)) && (!tc_shape || d.major != 10)) {
-        set_error("%s: tcgen05 path requested but unavailable (C=%d, sm_%d%d)", who, C, d.major, d.minor);
+    if ((flags & (MOCO_NCE_CTA_PAIR | MOCO_NCE_SINGLE_CTA)) && (!tc_shape || d.major != 9)) {
+        set_error("%s: tensor-core path requested but unavailable (C=%d, sm_%d%d)", who, C, d.major, d.minor);
         return MOCO_ERR_UNSUPPORTED;
     }
     cudaError_t e;
     bool prepped = false;
     // ---- one sweep over the queue for loss + gradient, then ONE tail kernel (merge, dq, optional enqueue)
-    const bool one_pass = want_tc && tc_shape && d.major == 10 && dq && !logits && !(flags & MOCO_NCE_TWO_PASS) &&
+    const bool one_pass = want_tc && tc_shape && d.major == 9 && dq && !logits && !(flags & MOCO_NCE_TWO_PASS) &&
                           ((flags & MOCO_NCE_ONE_PASS) || inv_T <= MOCO_ONE_PASS_MAX_INV_T) &&
                           !(normalize && C > 128);
     if (one_pass) {
@@ -156,7 +157,7 @@ static int nce_head(const void* q, const void* k, int qk_dtype, int normalize, c
             }
             return MOCO_OK;
         }
-        if (e != cudaErrorNotSupported) return cuda_fail("tcgen05 one-sweep kernel", e);
+        if (e != cudaErrorNotSupported) return cuda_fail("one-sweep kernel", e);
         // shape outside the one-sweep kernels' envelope: two-pass below
     }
     if (normalize || enq.index_dev) {
@@ -177,7 +178,7 @@ static int nce_head(const void* q, const void* k, int qk_dtype, int normalize, c
         }
         return MOCO_OK;
     };
-    if (want_tc && tc_shape && d.major == 10) {
+    if (want_tc && tc_shape && d.major == 9) {
         NceTcParams p;
         p.q_bf16 = qb; p.queue = queue; p.N = N; p.C = C; p.K = K; p.inv_T = inv_T; p.logits = logits;
         p.cta_group = (flags & MOCO_NCE_CTA_PAIR) ? 2 : 1;
@@ -194,14 +195,14 @@ static int nce_head(const void* q, const void* k, int qk_dtype, int normalize, c
                 prof_mark(MOCO_PROF_DQ, 0, stream);
                 e = launch_sweep(qb, MOCO_BF16, 0, qb, queue, N, C, K, inv_T, lse, d.sms, &slices, &n_pad, ws, stream);
                 prof_mark(MOCO_PROF_DQ, 1, stream);
-                if (e != cudaSuccess) return cuda_fail("tcgen05 dq kernel", e);
+                if (e != cudaSuccess) return cuda_fail("dq kernel", e);
                 e = launch_dq_reduce(N, C, slices, n_pad, inv_T, k, qk_dtype, prob_rows, dq, ws.part_o, stream);
                 if (e != cudaSuccess) return cuda_fail("dq reduce kernel", e);
             }
             return finish();
         }
         if (e != cudaErrorNotSupported || (flags & (MOCO_NCE_CTA_PAIR | MOCO_NCE_SINGLE_CTA)))
-            return cuda_fail("tcgen05 stats kernel", e);
+            return cuda_fail("statistics kernel", e);
         // shape outside the tensor-core kernel's envelope (e.g. N > 128 * #SM): generic path below
     }
     e = launch_simt_rows(qb, k, qk_dtype, queue, N, C, K, inv_T, logits, lse, loss_rows, prob_rows, loss_prob, dq, ws, stream);
@@ -319,8 +320,8 @@ static int shard_common(const char* what, const void* q, int N, int C, int Ks, v
     *ws = carve_workspace(workspace, N, C);
     if (bytes < ws->bytes) { set_error("%s: workspace too small (%zu < %zu)", what, bytes, ws->bytes); return MOCO_ERR_WORKSPACE; }
     *d = device_info();
-    if (!d->ok || d->major != 10 || C % 64 != 0 || C > 256) {
-        set_error("%s: needs an sm_100 device and C %% 64 == 0, C <= 256 (C=%d)", what, C);
+    if (!d->ok || d->major != 9 || C % 64 != 0 || C > 256) {
+        set_error("%s: needs an sm_90 device and C %% 64 == 0, C <= 256 (C=%d)", what, C);
         return MOCO_ERR_UNSUPPORTED;
     }
     return MOCO_OK;
@@ -348,10 +349,10 @@ int moco_nce_shard_stats(const void* q_all, const void* k_all, int qk_dtype, con
         // one sweep over the shard: (stabiliser, sum) partials for the cross-rank merge AND the unnormalised
         // P~.Queue partials, which stay in the workspace until moco_nce_shard_dq(..., MOCO_NCE_ONE_PASS) rescales them
         e = launch_sweep(q_all, qk_dtype, 0, p.q_bf16, p.queue, N, C, Ks, inv_T, nullptr, d.sms, &p.slices, &p.n_pad, ws, stream);
-        if (e != cudaSuccess) return cuda_fail("tcgen05 one-pass kernel", e);
+        if (e != cudaSuccess) return cuda_fail("one-pass kernel", e);
     } else {
         e = launch_nce_tc(p, ws, stream);
-        if (e != cudaSuccess) return cuda_fail("tcgen05 stats kernel", e);
+        if (e != cudaSuccess) return cuda_fail("statistics kernel", e);
     }
     e = launch_combine_partial(N, p.slices, p.n_pad, static_cast<float2*>(ms_out), ws, stream);
     if (e != cudaSuccess) return cuda_fail("combine kernel", e);
@@ -398,7 +399,7 @@ int moco_nce_shard_dq(const void* q_all, int q_dtype, const void* shard_bf16, co
     }
     e = launch_sweep(q_all, q_dtype, 0, qb, static_cast<const __nv_bfloat16*>(shard_bf16), N, C, Ks, inv_T, lse_all, d.sms, &slices,
                      &n_pad, ws, stream);
-    if (e != cudaSuccess) return cuda_fail("tcgen05 dq kernel", e);
+    if (e != cudaSuccess) return cuda_fail("dq kernel", e);
     e = launch_dq_reduce(N, C, slices, n_pad, inv_T, nullptr, 0, nullptr, o_partial, ws.part_o, stream);
     if (e != cudaSuccess) return cuda_fail("dq reduce kernel", e);
     return MOCO_OK;

@@ -8,8 +8,8 @@
 
 namespace moco {
 
-constexpr int kMaxCtas = 160;          // upper bound on persistent CTAs (B200: 148 SMs)
-constexpr int kRowsPerCta = 128;       // q rows per CTA in the tcgen05 kernels (UMMA M per CTA)
+constexpr int kMaxCtas = 160;          // upper bound on persistent CTAs (H100 SXM: 132 SMs)
+constexpr int kRowsPerCta = 128;       // q rows per CTA in the tensor-core kernels (two 64-row warpgroups)
 constexpr float kLog2e = 1.4426950408889634f;
 constexpr float kLn2 = 0.6931471805599453f;
 
@@ -113,28 +113,24 @@ cudaError_t launch_gather(const void* const* peers, int world, int rows_per_rank
 unsigned int* p2p_status_words();
 cudaError_t launch_signal_barrier(void* const* pads, int world, int rank, uint32_t epoch, cudaStream_t stream);
 
-// tcgen05 kernels (nce_sm100.cu).  Return cudaErrorNotSupported when the shape is not handled.
+// wgmma kernels (nce_sweep_sm90.cu).  Return cudaErrorNotSupported when the shape is not handled.
 struct NceTcParams {
     const __nv_bfloat16* q_bf16;   // [N, C]
     const __nv_bfloat16* queue;    // [K, C]
     int N, C, K;
     float inv_T;
     float* logits;                 // optional dense [N, K+1]
-    int cta_group;                 // 1 or 2
+    int cta_group;                 // 1, or 2: CTA pairs sharing every queue tile by TMA multicast
     int num_sms;
     // outputs of the launch decision
     int slices;
     int n_pad;
 };
 cudaError_t launch_nce_tc(NceTcParams& p, const NceWorkspace& ws, cudaStream_t stream);
-cudaError_t launch_nce_dq2_tc(const __nv_bfloat16* q_bf16, const __nv_bfloat16* queue, int N, int C, int K,
-                              float inv_T, const float* lse, int num_sms, int* slices_out,
-                              int* n_pad_out, const NceWorkspace& ws, cudaStream_t stream, bool plan_only = false);
-
-// one-sweep head for C in {64, 128} (nce_head128_sm100.cu) and the fused tail (nce_tail.cu)
-cudaError_t launch_nce_head128(const void* q, int q_dtype, int normalize, const __nv_bfloat16* queue, int N, int C, int K,
-                               float inv_T, const float* lse, int num_sms, int* slices_out, int* n_pad_out,
-                               const NceWorkspace& ws, cudaStream_t stream, bool plan_only = false);
+// the q.Queue^T sweep with the gradient partials (one-sweep mode when lse == nullptr) and the fused tail (nce_tail.cu)
+cudaError_t launch_nce_sweep(const void* q, int q_dtype, int normalize, const __nv_bfloat16* queue, int N, int C, int K,
+                             float inv_T, const float* lse, int num_sms, int* slices_out, int* n_pad_out,
+                             const NceWorkspace& ws, cudaStream_t stream, bool plan_only = false);
 bool nce_tail_can_enqueue(int C, int normalize);
 cudaError_t launch_nce_tail(int N, int C, int K, int slices, int n_pad, float inv_T, const void* q, const void* k,
                             int qk_dtype, int normalize, const __nv_bfloat16* queue, float* lse, float* loss_rows,

@@ -95,7 +95,7 @@ int ema_chunk_elems() { return kEmaChunk; }
 cudaError_t launch_ema(const void* segs, const int* chunk_prefix, int n_segs, int n_chunks, float m, float one_minus_m,
                        cudaStream_t stream) {
     if (n_segs == 0 || n_chunks == 0) return cudaSuccess;
-    int blocks = n_chunks < 148 * 8 ? n_chunks : 148 * 8;
+    int blocks = n_chunks < 132 * 8 ? n_chunks : 132 * 8;
     ema_multi_kernel<<<blocks, kEmaThreads, 0, stream>>>(static_cast<const EmaSeg*>(segs), chunk_prefix, n_segs, n_chunks,
                                                          m, one_minus_m);
     return cudaGetLastError();

@@ -3,7 +3,7 @@
 // against the whole queue (the generic path, and the fallback for rows the one-sweep kernel cannot represent).
 #pragma once
 #include "common.cuh"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace moco {
 

@@ -1,13 +1,13 @@
 // Support kernels of the InfoNCE head: prep (positive logit + bf16 cast of q),
 // the cross-slice combine (lse / loss / prob / dq), the generic CUDA-core
-// row kernel (any shape; also the on-GPU cross-check of the tcgen05 kernels) and
+// row kernel (any shape; also the on-GPU cross-check of the tensor-core kernels) and
 // the dense-gradient backward of the compatibility API.
 //
 // Reference semantics: moco/NCE/Contrast.py:20-27, moco/NCE/NCECriterion.py:11-13,
 // train.py:264,273 (see include/moco_b200.h).
 #include "common.cuh"
 #include "nce_rows.cuh"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace moco {
 
@@ -44,7 +44,7 @@ cudaError_t launch_prep(const void* q, const void* k, int qk_dtype, int N, int C
 }
 
 // ---------------------------------------------------------------------------
-// combine: merge the per-slice (max, sum[, O]) partials of the tcgen05 kernel.
+// combine: merge the per-slice (max, sum[, O]) partials of the tensor-core kernel.
 // One block per q row.
 // ---------------------------------------------------------------------------
 __global__ void combine_kernel(int N, int C, int K, int slices, int n_pad, float inv_T,

@@ -1,4 +1,4 @@
-// Tail of the one-sweep InfoNCE head: everything after the tcgen05 kernel in ONE launch.
+// Tail of the one-sweep InfoNCE head: everything after the sweep kernel in ONE launch.
 //
 //   blocks [0, N)        one per query row: positive logit <q_i, k_i> (fp32, from the inputs as given, optionally
 //                        L2-normalised here), merge of the per-slice (stabiliser, sum) pairs -> lse / loss_i / prob_i
@@ -28,15 +28,9 @@
 #include "../../include/moco_b200.h"
 #include "common.cuh"
 #include "nce_rows.cuh"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace moco {
-
-#ifdef MOCO_TRACE
-__device__ unsigned long long g_tail_evt[64][4];       // per launch: [2] first block past pdl_wait, [3] last exit
-__device__ unsigned int g_tail_launch = 0;
-__device__ __forceinline__ unsigned long long tail_gtime() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
-#endif
 
 constexpr int kTailThreads = kSimtThreads;         // 256
 constexpr int kMaxTailDevices = 64;
@@ -78,9 +72,6 @@ nce_tail_kernel(const TailArgs a) {
     __shared__ float s_val[4];                     // lse2, prob, unsafe flag
     pdl_wait();                                    // the head kernel has completed; see the header comment
     const int tid = threadIdx.x;
-#ifdef MOCO_TRACE
-    if (tid == 0) atomicMin(&g_tail_evt[g_tail_launch & 63u][2], tail_gtime());
-#endif
     const long long ring = a.index_dev ? *a.index_dev : a.index;
     if ((int)blockIdx.x < a.N) {
         const int i = blockIdx.x;
@@ -299,10 +290,6 @@ nce_tail_kernel(const TailArgs a) {
         }
     }
     const bool last = finish_mean(a.counters + 0, a.N, a.loss_rows, a.prob_rows, a.loss_prob);
-#ifdef MOCO_TRACE
-    if (tid == 0) atomicMax(&g_tail_evt[g_tail_launch & 63u][3], tail_gtime());
-    if (last && tid == 0) { __threadfence(); g_tail_launch = g_tail_launch + 1u; }
-#endif
     if (last && tid == 0) {
         a.counters[1] = 0u;                               // re-arm (every enqueue block has passed its wait: it arrived here)
         if (a.index_dev != nullptr && a.n_all > 0) *a.index_dev = (ring + a.n_all) % a.K;
@@ -340,7 +327,7 @@ cudaError_t launch_nce_tail(int N, int C, int K, int slices, int n_pad, float in
         if (!nce_tail_can_enqueue(C, normalize)) return cudaErrorNotSupported;
         const int rows_per_pass = kTailThreads / vec_per_row;
         a.enq_blocks = (n_all + rows_per_pass - 1) / rows_per_pass;
-        if (a.enq_blocks > 148) a.enq_blocks = 148;
+        if (a.enq_blocks > 132) a.enq_blocks = 132;
     }
     // same shared-memory carve-out as the 227 KB head kernel in front of it: no SM reconfiguration between the two
     static bool carveout_set[kMaxTailDevices] = {false};
@@ -352,17 +339,5 @@ cudaError_t launch_nce_tail(int N, int C, int K, int slices, int n_pad, float in
     return launch_pdl(nce_tail_kernel, dim3(N + a.enq_blocks), dim3(kTailThreads), 0, stream, a);
 }
 
-#ifdef MOCO_TRACE
-extern "C" int moco_debug_tail_evt(unsigned long long* host_buf) {
-    return (int)cudaMemcpyFromSymbol(host_buf, g_tail_evt, sizeof(g_tail_evt));
-}
-extern "C" int moco_debug_tail_evt_reset() {
-    static unsigned long long init[64][4];
-    for (int i = 0; i < 64; ++i) { init[i][0] = ~0ull; init[i][1] = 0; init[i][2] = ~0ull; init[i][3] = 0; }
-    unsigned int z = 0;
-    cudaMemcpyToSymbol(g_tail_launch, &z, sizeof(z));
-    return (int)cudaMemcpyToSymbol(g_tail_evt, init, sizeof(init));
-}
-#endif
 
 }  // namespace moco

@@ -1,8 +1,6 @@
 // 3x3 / stride 2 / pad 1 max pooling of the stem's channels_last bf16 activation (reference: moco/models/resnet.py:119,158
-// `nn.MaxPool2d(kernel_size=3, stride=2, padding=1)`), forward and backward.  With the BatchNorm group on this
-// library's kernels ATen's max_pool_forward_nhwc / max_pool_backward_nhwc were 8 % of the step (0.75 ms per forward,
-// 1.7 ms per backward for a 411 MB input; profiles/r2_bench_launches_by_kernel_fused_bn.csv) for what is one read of
-// the input and one write of a quarter-size output.
+// `nn.MaxPool2d(kernel_size=3, stride=2, padding=1)`), forward and backward: one read of the input and one write of
+// a quarter-size output.
 //
 // Semantics = torch.nn.functional.max_pool2d: out-of-image taps are skipped, the window is scanned kh then kw and
 // the FIRST maximum wins (`val > max || isnan(val)`), which matters here because post-ReLU windows are full of equal

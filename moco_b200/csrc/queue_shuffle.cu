@@ -3,7 +3,7 @@
 // cross-GPU signal barrier.  All HBM/NVLink-bound byte movers: 16-byte vector
 // accesses, bulk-async (TMA) copies for large rows, grids sized from the SM count.
 #include "common.cuh"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace moco {
 
@@ -71,13 +71,13 @@ cudaError_t launch_enqueue(__nv_bfloat16* queue_bf16, float* queue_f32, const vo
     if ((C & 7) == 0) {
         long long total = (long long)n_all * (C >> 3);
         int blocks = (int)((total + 255) / 256);
-        if (blocks > 148 * 8) blocks = 148 * 8;
+        if (blocks > 132 * 8) blocks = 132 * 8;
         return launch_pdl(enqueue_kernel, dim3(blocks), dim3(256), 0, stream, queue_bf16, queue_f32, k_all, k_dtype, n_all, C,
                           (long long)K, (long long)index, (long long)row0, (long long)nrows);
     } else {
         long long total = (long long)n_all * C;
         int blocks = (int)((total + 255) / 256);
-        if (blocks > 148 * 8) blocks = 148 * 8;
+        if (blocks > 132 * 8) blocks = 132 * 8;
         return launch_pdl(enqueue_scalar_kernel, dim3(blocks), dim3(256), 0, stream, queue_bf16, queue_f32, k_all, k_dtype,
                           n_all, C, (long long)K, (long long)index, (long long)row0, (long long)nrows);
     }
@@ -102,7 +102,7 @@ __global__ void f32_to_bf16_kernel(const float* __restrict__ src, __nv_bfloat16*
 cudaError_t launch_f32_to_bf16(const float* src, __nv_bfloat16* dst, size_t n, cudaStream_t stream) {
     if (n == 0) return cudaSuccess;
     size_t blocks = (n / 4 + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     if (blocks == 0) blocks = 1;
     f32_to_bf16_kernel<<<(int)blocks, 256, 0, stream>>>(src, dst, n);
     return cudaGetLastError();
@@ -236,7 +236,7 @@ gather_bulk_kernel(PeerTable peers, SyncArgs sa, int rows_per_rank, const int64_
     const unsigned long long mine = first < total ? (total - first + stride - 1) / stride : 0ull;     // items of this CTA
     auto item = [&](unsigned long long k, const char*& s, char*& d, uint32_t& bytes) {
         // chunk-major order: consecutive CTAs work on consecutive ROWS (rows of a shuffled batch live on different
-        // peers), so at any moment the pulls are spread over all source GPUs instead of 148 CTAs draining one row
+        // peers), so at any moment the pulls are spread over all source GPUs instead of 132 CTAs draining one row
         const unsigned long long it = first + k * stride;
         const unsigned long long row = it % (unsigned long long)n_rows, ch = it / (unsigned long long)n_rows;
         const long long g = src_rows[row];
@@ -336,9 +336,8 @@ cudaError_t launch_gather(const void* const* peers_host, int world, int rows_per
     }
     PeerTable t;
     for (int i = 0; i < kMaxWorld; ++i) t.base[i] = i < world ? static_cast<const char*>(peers_host[i]) : nullptr;
-    // AUTO: bulk-async copies for rows up to ~300 KB (bf16 images: 152.7 vs 157.5 us at 8 GPUs, and one thread per SM
-    // instead of 8 warps), the 16-byte load/store kernel above that (fp32 images, 602 KB rows: 286 vs 342 us) --
-    // profiles/r2_multi_gpu8_check.json
+    // AUTO: bulk-async copies for rows up to ~400 KB (bf16 images; one thread per SM instead of 8 warps), the 16-byte
+    // load/store kernel above that (fp32 images, 602 KB rows)
     const bool use_ldg = (flags & 1) || row_bytes > (size_t)400 * 1024;
     if (row_bytes >= (size_t)kChunk / 2 && use_ldg) {
         if (sa.epoch != 0u) signal_barrier_kernel<<<1, 32, 0, stream>>>(sa);
@@ -358,7 +357,7 @@ cudaError_t launch_gather(const void* const* peers_host, int world, int rows_per
             attr_set[dev] = true;
         }
         size_t chunks = (row_bytes + kChunk - 1) / kChunk * (size_t)n_rows;
-        int grid = (int)(chunks < 148 ? chunks : 148);
+        int grid = (int)(chunks < 132 ? chunks : 132);
         gather_bulk_kernel<<<grid, 32, smem, stream>>>(t, sa, rows_per_rank, src_rows, n_rows, row_bytes,
                                                        static_cast<char*>(dst));
     } else {
@@ -436,7 +435,7 @@ crop_to_nhwc_kernel(const SrcT* __restrict__ src, long long img_stride, __nv_bfl
 // (moco/models/resnet.py:112, 7x7 / stride 2 / pad 3 on 3 channels) equals a 4x4 / stride 1 / pad 0 convolution over
 //     s[n, R, Q, (b * 2 + d) * 3 + c] = x[n, c, 2 (R - 2) + b, 2 (Q - 2) + d]     (0 outside the image; channels 12..15 = 0)
 // with R < H/2 + 3, Q < W/2 + 3 (two zero rows / columns in front, one behind: the 7-tap window padded to 8 taps),
-// and 16 input channels are what cuDNN's sm_100 implicit-GEMM kernels want (C = 3 runs a legacy kernel at 2 % of
+// and 16 input channels are what cuDNN's implicit-GEMM kernels want (C = 3 runs a legacy kernel at 2 % of
 // peak plus channel-padding passes).  One thread per output pixel: 6 coalesced 8-byte (fp32) or 4-byte (bf16) loads,
 // two 16-byte stores.
 template <typename SrcT>
@@ -486,7 +485,7 @@ cudaError_t launch_crop_to_s2d(const void* src, int src_dtype, long long img_str
     if (H < 2 || W < 2 || (H & 1) || (W & 1)) return cudaErrorNotSupported;
     const long long total = (long long)N * ((H >> 1) + 3) * ((W >> 1) + 3);
     long long blocks = (total + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
     if (src_dtype == 0)
         return launch_pdl(crop_to_s2d_kernel<float>, dim3((unsigned)blocks), dim3(256), 0, stream,
                           static_cast<const float*>(src), img_stride, dst, N, H, W, src_rows);
@@ -500,7 +499,7 @@ cudaError_t launch_crop_to_nhwc(const void* src, int src_dtype, long long img_st
     if (C < 1 || C > 4 || (HW & 7) != 0) return cudaErrorNotSupported;
     const long long total = (long long)N * (HW >> 3);
     long long blocks = (total + 255) / 256;
-    if (blocks > 148 * 16) blocks = 148 * 16;
+    if (blocks > 132 * 16) blocks = 132 * 16;
 #define MOCO_CROP(C_)                                                                                                 \
     if (C == C_) {                                                                                                    \
         if (src_dtype == 0)                                                                                           \

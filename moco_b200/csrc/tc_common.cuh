@@ -1,5 +1,5 @@
-// Shared pieces of the tcgen05 kernels' translation units: smem constants, tensor-map creation, and the
-// persistent-grid launch planner (cluster-aware).
+// Shared pieces of the tensor-core (wgmma) kernels' translation units: smem constants, tensor-map creation, and
+// the persistent-grid launch planner (cluster-aware).
 #pragma once
 #include <cuda.h>
 #include <stdlib.h>
@@ -7,12 +7,12 @@
 #include <mutex>
 
 #include "common.cuh"
-#include "sm100_ptx.cuh"
+#include "sm90_ptx.cuh"
 
 namespace moco {
 
 constexpr int kSlab = 128 * 128;            // bytes of a [128 rows x 64 bf16] swizzled slab
-constexpr int kSmemBudget = 232448 - 1024;  // max dynamic smem per CTA minus alignment slack
+constexpr int kSmemBudget = 232448 - 1024;  // max dynamic smem per CTA on sm_90 (227 KB) minus alignment slack
 
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
@@ -50,8 +50,8 @@ inline bool make_tmap(CUtensorMap* m, const void* base, int rows, int C, int box
 }
 
 // Per-kernel launch state: the max-dynamic-smem attribute is set once, and the number of clusters that can be
-// co-resident (persistent grid: one wave) is queried once per (smem, cluster) -- cluster size 4 strands SMs
-// in GPCs whose SM count is not a multiple of 4, so it is NOT simply #SM / cluster.
+// co-resident (persistent grid: one wave) is queried once per (smem, cluster) -- a cluster size > 1 can strand SMs
+// in GPCs whose SM count is not a multiple of it, so it is NOT simply #SM / cluster.
 struct KernelCache {
     int smem_set = -1;
     int q_smem = -1, q_cluster = -1, q_result = 0;
@@ -59,7 +59,7 @@ struct KernelCache {
 
 // cudaFuncSetAttribute and the occupancy answer are per DEVICE: one cache entry per (device ordinal, kernel slot of
 // this translation unit), all guarded by one mutex (launches from several host threads / several GPUs in one process).
-constexpr int kMaxDevices = 64, kCacheSlots = 8;
+constexpr int kMaxDevices = 64, kCacheSlots = 32;
 static std::mutex g_kernel_cache_mutex;
 static KernelCache& kernel_cache(int slot) {
     static KernelCache table[kMaxDevices][kCacheSlots];
@@ -103,7 +103,7 @@ static cudaError_t prepare_kernel(Kern kern, KernelCache& kc, int threads, int s
 
 template <typename Kern, typename Args>
 static cudaError_t launch_cluster(Kern kern, int grid, int threads, int smem, int cluster, cudaStream_t stream,
-                                  const CUtensorMap& a, const CUtensorMap& b, const Args& args, bool pdl = false) {
+                                  const CUtensorMap& tmap, const Args& args, bool pdl = false) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(grid);
     cfg.blockDim = dim3(threads);
@@ -125,14 +125,14 @@ static cudaError_t launch_cluster(Kern kern, int grid, int threads, int smem, in
     }
     cfg.attrs = attr;
     cfg.numAttrs = n;
-    return cudaLaunchKernelEx(&cfg, kern, a, b, args);
+    return cudaLaunchKernelEx(&cfg, kern, tmap, args);
 }
 
 // plan + launch one templated kernel instance: `fill(slices)` finalises the argument struct
 template <typename Kern, typename Args, typename Fill>
 static cudaError_t plan_and_launch(Kern kern, KernelCache& kc, int threads, int smem, int cluster, int mgroups,
                                    int ctas_per_slice, int num_tiles, int n_pad, int* slices_out, cudaStream_t stream,
-                                   const CUtensorMap& a, const CUtensorMap& b, Args& args, Fill fill, bool pdl = false,
+                                   const CUtensorMap& tmap, Args& args, Fill fill, bool pdl = false,
                                    bool plan_only = false) {
     int max_clusters = 0;
     cudaError_t e;
@@ -149,14 +149,7 @@ static cudaError_t plan_and_launch(Kern kern, KernelCache& kc, int threads, int 
     *slices_out = slices;
     if (plan_only) return cudaSuccess;          // the caller only needs the (deterministic) slice count
     fill(args, slices);
-    return launch_cluster(kern, ctas_per_slice * slices, threads, smem, cluster, stream, a, b, args, pdl);
-}
-
-// bring-up switch for pipeline experiments (never set in production): see StatsArgs::debug
-inline int debug_mode() {
-    static int v = -1;
-    if (v < 0) { const char* e = getenv("MOCO_DEBUG_MODE"); v = e ? atoi(e) : 0; }
-    return v;
+    return launch_cluster(kern, ctas_per_slice * slices, threads, smem, cluster, stream, tmap, args, pdl);
 }
 
 }  // namespace moco

@@ -65,7 +65,7 @@ class StemConv(nn.Conv2d):
     space-to-depth input that ``moco_crop_s2d_bf16`` writes ([N, 16, H/2+3, W/2+3], see include/moco_b200.h) it runs
     the EQUIVALENT 4x4 / stride 1 convolution with the weights re-indexed on the fly,
         w'[o, (b*2+d)*3 + c, a, e] = w[o, c, 2a+b-1, 2e+d-1]        (taps -1 are zero),
-    which is differentiable w.r.t. the 7x7 parameter -- so cuDNN sees 16 input channels (its sm_100 implicit-GEMM
+    which is differentiable w.r.t. the 7x7 parameter -- so cuDNN sees 16 input channels (its implicit-GEMM
     kernels) instead of 3 (a legacy kernel at 2 % of peak + channel-padding passes)."""
 
     def __init__(self):

@@ -1,5 +1,5 @@
 """One MoCo pretraining iteration -- the body of ``train_moco`` (train.py:244-283 of bl0/moco)
-with the contrastive hot path on the sm_100a kernels.
+with the contrastive hot path on the sm_90a kernels.
 
 Differences from the reference loop body, none of which change the math:
 * the ShuffleBN image permute runs on a side stream, overlapped with the query-encoder forward;

@@ -5,7 +5,7 @@ Same public names and semantics as the reference (``util.py:47-111``):
 get_local_id, get_shuffle_ids}``; plus ``set_bn_train`` / ``moment_update``
 (``util.py:114-127``) which the training step needs.
 
-B200-native design: the reference all_gathers every rank's whole batch (W x the
+Native design: the reference all_gathers every rank's whole batch (W x the
 bytes it needs, plus a zero-fill and a cat of the same size, util.py:55-58) and
 then indexes it.  Here each rank publishes its batch in a peer-mapped staging
 buffer and every rank PULLS exactly the rows its slice of the permutation names,

@@ -330,8 +330,8 @@ def moment_update(params: Sequence[np.ndarray], params_ema: Sequence[np.ndarray]
 def one_sweep_head(q: np.ndarray, k: np.ndarray, memory_pre: np.ndarray, T: float, tile: int = 128,
                    slices: int = 4) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
     """lse, prob and dq of the reference head (Contrast.py:20-27, NCECriterion.py:11-13, train.py:264,273)
-    computed the way ``nce_dq2_kernel<FUSED>`` does: the queue is cut into `slices` runs of `tile`-row tiles;
-    every (slice, row) keeps the row maximum of its FIRST tile as a fixed stabiliser m and accumulates
+    computed the way a one-sweep kernel with a per-slice stabiliser does: the queue is cut into `slices` runs of
+    `tile`-row tiles; every (slice, row) keeps the row maximum of its FIRST tile as a fixed stabiliser m and accumulates
     l = sum 2^(x - m) and O = sum 2^(x - m) queue_j in fp32 with no rescaling; slices are merged afterwards.
     Mathematically identical to logsumexp / softmax-weighted sum; in fp32 it overflows (inf) when a later logit
     exceeds the first tile's maximum by more than ~88 nats -- exactly the CUDA kernel's documented contract."""

@@ -7,7 +7,7 @@ path: models are the reference's own ``moco.models.resnet``, the head is its ``m
 ``NCESoftmaxLoss``, ShuffleBN its ``DistributedShufle`` over a gloo process group, the optimizer / scheduler /
 EMA exactly what ``train.main`` builds (train.py:175-198).
 
-Shims (BASELINE.md section 4; none touches a reference file):
+Shims (none touches a reference file):
   1. identity ``torch.Tensor.cuda`` / ``nn.Module.cuda`` -- the reference hard-codes ``.cuda()``
      (Contrast.py:32, util.py:104-108, train.py:253-254);
   2. a stub ``termcolor`` module (moco/logger.py:6 imports it; the package is not installed);

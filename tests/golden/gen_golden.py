@@ -91,7 +91,9 @@ def gen_contrast():
     sd = MemoryMoCo(128, 16, 0.07).state_dict()
     out["state_dict_keys"] = np.array(sorted(sd.keys()))
     out["state_dict_params"] = sd["params"].numpy()
-    np.savez_compressed(os.path.join(OUT, "contrast.npz"), **out)
+    # split so that every fixture file stays under 1 MB (tests/helpers.py:load_contrast_golden merges them)
+    np.savez_compressed(os.path.join(OUT, "contrast_c1head.npz"), **{k: v for k, v in out.items() if k.startswith("c1head_")})
+    np.savez_compressed(os.path.join(OUT, "contrast.npz"), **{k: v for k, v in out.items() if not k.startswith("c1head_")})
 
 
 # ------------------------------------------------------------------ Normalize -> head (SURVEY 8 f2)

@@ -1,4 +1,6 @@
-"""Test helpers: oracle evaluation in K-chunks (memory-light at full BASELINE sizes)."""
+"""Test helpers: oracle evaluation in K-chunks (memory-light at full BASELINE sizes), golden-vector loading."""
+import os
+
 import numpy as np
 
 from oracle import moco_oracle as O
@@ -32,3 +34,15 @@ def oracle_head_chunked(q, k, memory, T, chunk=16384, want_dq=True):
 def rand_unit(rng, n, c):
     x = rng.standard_normal((n, c)).astype(np.float32)
     return O.bf16_round(O.l2_normalize(x))
+
+
+CONTRAST_GOLDEN = ("contrast.npz", "contrast_c1head.npz")      # one set of vectors, split to keep each file < 1 MB
+
+
+def load_contrast_golden(golden_dir):
+    """The reference's MemoryMoCo / NCESoftmaxLoss vectors (tests/golden/gen_golden.py:gen_contrast) as one mapping."""
+    out = {}
+    for name in CONTRAST_GOLDEN:
+        with np.load(os.path.join(golden_dir, name)) as z:
+            out.update({k: z[k] for k in z.files})
+    return out

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with ``-m gpu`` on a B200): the CUDA path, called through the C ABI
+"""GPU parity tests (run with ``-m gpu`` on an H100): the CUDA path, called through the C ABI
 (ctypes -> libmoco_b200.so) by the Python mirror of the reference API, against
 (a) the golden vectors produced by the unmodified reference and (b) the numpy oracle on seeded
 inputs.  Tolerances: logits 1e-3 relative to max|logit| (BASELINE.json north_star) on identical
@@ -10,7 +10,7 @@ import pytest
 import torch
 
 from oracle import moco_oracle as O
-from tests.helpers import oracle_head_chunked, rand_unit
+from tests.helpers import load_contrast_golden, oracle_head_chunked, rand_unit
 
 pytestmark = pytest.mark.gpu
 
@@ -24,13 +24,13 @@ def _flags():
     return {"auto": _lib.NCE_AUTO, "simt": _lib.NCE_FORCE_SIMT, "tc1": _lib.NCE_SINGLE_CTA,
             # one sweep for loss + dq (what AUTO picks at MoCo temperatures) vs statistics pass + dq pass
             "onepass": _lib.NCE_SINGLE_CTA | _lib.NCE_ONE_PASS, "twopass": _lib.NCE_SINGLE_CTA | TP,
-            # CTA-pair statistics kernel (the one round-1 alternative that measured faster; the losers were removed)
+            # statistics kernel on CTA pairs that share every queue tile (TMA multicast)
             "tc2": _lib.NCE_CTA_PAIR | TP}
 
 
 @pytest.fixture(scope="module")
 def contrast_golden(golden_dir):
-    return np.load(os.path.join(golden_dir, "contrast.npz"))
+    return load_contrast_golden(golden_dir)
 
 
 def test_library_is_the_cuda_one():
@@ -39,7 +39,7 @@ def test_library_is_the_cuda_one():
     import ctypes
     sm, major = ctypes.c_int(), ctypes.c_int()
     assert lib.moco_device_info(ctypes.byref(sm), ctypes.byref(major), None) == 0
-    assert major.value == 10 and sm.value >= 100, "expected a Blackwell (sm_100) device"
+    assert major.value == 9 and sm.value >= 100, "expected a Hopper (sm_90) device"
 
 
 @pytest.mark.parametrize("flag", ["auto", "simt", "tc1", "tc2"])
@@ -175,7 +175,7 @@ def test_low_temperature_both_sweeps(flag):
     before = _lib.launches
     l, p, g = _head_gpu(q, k, memory, T, _flags()[flag])
     n_launch = _lib.launches - before - 1                # minus f32->bf16 of the queue
-    # one sweep: the tcgen05 kernel + ONE tail kernel that also enqueues; two-pass: prep, stats, combine, dq,
+    # one sweep: the sweep kernel + ONE tail kernel that also enqueues; two-pass: prep, stats, combine, dq,
     # dq_reduce + the enqueue kernel
     assert n_launch == (2 if flag == "onepass" else 6), n_launch
     assert abs(l - loss) < 2e-4 * max(1.0, abs(loss)), (l, loss)
@@ -281,7 +281,7 @@ def test_fp32_inputs_are_rounded_to_bf16_exactly_once():
     negatives = <bf16(q), bf16(queue)> with fp32 accumulation, positive = <q, k> in fp32.  Against the
     oracle fed the same rounded operands the logits are tight (north_star: 1e-3 relative on identical
     inputs); against the un-rounded fp32 oracle the only difference is the bf16 operand quantisation
-    (2^-9 per element), bounded here and quantified in DESIGN.md."""
+    (2^-9 per element), bounded here."""
     from moco_b200.NCE import MemoryMoCo
     rng = np.random.default_rng(5)
     N, C, K, T = 64, 128, 4096, 0.07
@@ -708,7 +708,9 @@ def test_step_with_fused_input_path_matches_plain_step():
         ema = encoders.resnet18(low_dim=128).cuda().to(memory_format=torch.channels_last)
         ema.load_state_dict(model.state_dict())
         contrast = MemoryMoCo(128, 1024, 0.07).cuda()
-        opt = torch.optim.SGD(model.parameters(), lr=0.03, momentum=0.9, weight_decay=1e-4)
+        # lr 0.003: two SGD steps at 0.03 on 16 images turn a last-bit difference of the first convolution's cuDNN
+        # kernels into a few % of loss by step 3 (seen with H100's kernels), which the bounds below would not hold
+        opt = torch.optim.SGD(model.parameters(), lr=0.003, momentum=0.9, weight_decay=1e-4)
         step = MoCoStep(model, ema, contrast, opt, channels_last=nhwc)
         g = torch.Generator(device="cuda").manual_seed(4)
         out = []
@@ -781,7 +783,7 @@ def test_step_with_fused_normalize_and_graphed_tail_matches_plain_step(graph):
 
 
 def test_normalize_falls_back_to_torch_where_the_kernels_do_not_fuse_it():
-    """feat_dim 256 runs on nce_head256_kernel, which takes q already normalised: forward_loss(normalize=True)
+    """feat_dim 256 runs on nce_sweep_kernel<4, ...>, which takes q already normalised: forward_loss(normalize=True)
     then normalises in torch (same definition as resnet.py:30-33) -- same result contract, three more launches."""
     from moco_b200.NCE import MemoryMoCo
     rng = np.random.default_rng(31)

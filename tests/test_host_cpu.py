@@ -37,8 +37,8 @@ def test_library_exports_every_declared_symbol():
     assert lib.moco_nce_workspace_bytes(256, 128, 16384) > 0
 
 
-def test_library_is_sm100a_native():
-    """The shipped .so carries sm_100a SASS with tcgen05 / TMA instructions (no PTX JIT, no fallback arch)."""
+def test_library_is_sm90a_native():
+    """The shipped .so carries sm_90a SASS with wgmma / TMA / mbarrier instructions (no PTX JIT, no fallback arch)."""
     import shutil
     import subprocess
     from moco_b200 import _lib
@@ -46,8 +46,8 @@ def test_library_is_sm100a_native():
     if not os.path.exists(cuobjdump):
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([cuobjdump, "-sass", _lib.lib_path()], capture_output=True, text=True).stdout
-    assert "sm_100a" in sass
-    for mnemonic in ("UTCHMMA", "UTMALDG", "LDTM", "UBLKCP"):
+    assert "sm_90a" in sass and "sm_100" not in sass
+    for mnemonic in ("HGMMA", "UTMALDG", "SYNCS", "UBLKCP"):
         assert mnemonic in sass, mnemonic
 
 

@@ -7,6 +7,7 @@ import pytest
 import torch
 
 from oracle import moco_oracle as O
+from tests.helpers import load_contrast_golden
 
 
 @pytest.fixture(scope="module")
@@ -16,7 +17,7 @@ def ids(golden_dir):
 
 @pytest.fixture(scope="module")
 def contrast(golden_dir):
-    return np.load(os.path.join(golden_dir, "contrast.npz"))
+    return load_contrast_golden(golden_dir)
 
 
 @pytest.fixture(scope="module")
@@ -236,6 +237,27 @@ def test_space_to_depth_stem_is_the_reference_conv1(golden_dir):
         _close(stem(torch.from_numpy(xs)).numpy(), g["stem_conv1"], 2e-5, 2e-5)
         _close(stem(torch.from_numpy(g["stem_x"])).numpy(), g["stem_conv1"], 2e-5, 2e-5)
 
+
+
+def test_stem_conv_s2d_weight_gradient_is_the_7x7_gradient():
+    """The gradient StemConv's 4x4 space-to-depth form sends back through its re-indexed weights is the 7x7 / 2 / pad 3
+    convolution's weight gradient, in fp32 on CPU (no cuDNN, no bf16): an error in the re-indexing shows at O(1)."""
+    import torch.nn.functional as F
+    from oracle import encoder_ops_oracle as E
+    from moco_b200.encoders import StemConv
+    g = torch.Generator().manual_seed(5)
+    x = torch.randn(2, 3, 30, 34, generator=g)
+    dy = torch.randn(2, 64, 15, 17, generator=g)
+    stem = StemConv()
+    y_s2d = stem(torch.from_numpy(E.s2d_layout(x.numpy())))
+    y_s2d.backward(dy)
+    g_s2d = stem.weight.grad.clone()
+    w = stem.weight.detach().clone().requires_grad_(True)
+    y_ref = F.conv2d(x, w, None, 2, 3)
+    y_ref.backward(dy)
+    assert y_s2d.shape == y_ref.shape
+    assert float((y_s2d - y_ref).detach().abs().max()) < 1e-5 * float(y_ref.detach().abs().max())
+    assert float((g_s2d - w.grad).abs().max()) < 1e-5 * float(w.grad.abs().max())
 
 def test_norm_modules_off_the_gpu_reproduce_the_reference_modules(golden_dir):
     """BatchNormAct2d / MaxPool3x3s2 on CPU tensors (their torch path) against the same captured tensors."""

@@ -138,7 +138,7 @@ def run_nce(name):
         out["dq_tflops"] = 4.0 * N * C * K / (out["dq_kernel_us"] * 1e-6) / 1e12
         import ctypes
         win = ctypes.c_float()
-        lib.moco_prof_sweep_window(ws_ptr, 148, ctypes.byref(win), stream)
+        lib.moco_prof_sweep_window(ws_ptr, torch.cuda.get_device_properties(0).multi_processor_count, ctypes.byref(win), stream)
         out["sweep_device_window_us"] = float(win.value)
     return out
 
@@ -209,7 +209,8 @@ def run_module(name):
     import numpy as np
     import torch
     from moco_b200.NCE import MemoryMoCo, NCESoftmaxLoss
-    g = np.load(os.path.join(ROOT, "tests", "golden", "contrast.npz"))
+    from tests.helpers import load_contrast_golden
+    g = load_contrast_golden(os.path.join(ROOT, "tests", "golden"))
     res = {"case": name, "ok": True}
     for cname in ["c1head", "wrap", "c256", "ragged"]:
         N, C, K, A, steps = (int(v) for v in g[f"{cname}_meta"])

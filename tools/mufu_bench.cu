@@ -1,5 +1,5 @@
-// Microbenchmark: per-SM throughput of the exp2 paths the NCE epilogue can use (B200).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o /tmp/mufu_bench tools/mufu_bench.cu && /tmp/mufu_bench
+// Microbenchmark: per-SM throughput of the exp2 paths the NCE epilogue can use (H100).
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o /tmp/mufu_bench tools/mufu_bench.cu && /tmp/mufu_bench
 #include <cstdio>
 #include <cuda_fp16.h>
 #include <cuda_bf16.h>
@@ -53,7 +53,7 @@ __global__ void k(float* out, int iters, float seed) {
 
 template <int MODE>
 void run(const char* name, int threads) {
-    int sms = 148, iters = 4096;
+    int sms = 132, iters = 4096;
     float* out;
     cudaMalloc(&out, sizeof(float) * sms * threads);
     cudaEvent_t e0, e1;

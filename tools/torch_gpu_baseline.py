@@ -1,4 +1,4 @@
-"""SURVEY.md §8(d): "the reference PyTorch path on the same B200 as the primary beat-this baseline for every
+"""SURVEY.md §8(d): "the reference PyTorch path on the same GPU as the primary beat-this baseline for every
 kernel".  Times, on one GPU with CUDA events, the post-encoder head (a7-a11: logits + loss + prob + backward to
 q + enqueue) and the EMA update (f1) two ways:
 
