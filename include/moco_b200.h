@@ -269,6 +269,62 @@ int moco_bn_bwd(const void* dy, const void* x, const void* y_or_null, long long 
                 int relu, int has_residual, void* dx, void* dresidual_or_null, float* dgamma, float* dbeta,
                 void* workspace, size_t workspace_bytes, void* stream);
 
+/* The residual BatchNorm of a block, relu(bn(x) + r), with the ReLU mask kept as bits and, in a downsample block,
+ * the shortcut's BatchNorm folded in.  Same arithmetic, roundings and reductions as moco_bn_fwd_train /
+ * moco_bn_bwd: the results are bit-identical to those calls, with fewer bytes moved.
+ *
+ * moco_bn_layer: one BatchNorm's tensors.  gamma, beta, running_*, save_*, dgamma, dbeta: fp32 [C];
+ * running_mean/var (both or neither) and num_batches_tracked may be NULL; momentum and eps as in
+ * moco_bn_fwd_train.  The forward writes save_mean / save_invstd; the backward reads gamma and save_* and
+ * writes dgamma / dbeta (beta, running_* and num_batches_tracked are not used there).
+ *
+ * moco_bn_add_relu_fwd_train: y = relu(bn(x) + r) with
+ *     r = residual                                  when shortcut == NULL (identity shortcut),
+ *     r = bf16(shortcut_bn(residual))               otherwise: residual is the shortcut convolution's raw output,
+ *                                                   normalised with its own batch statistics (running statistics
+ *                                                   updated as moco_bn_fwd_train does), rounded to bf16 as the
+ *                                                   materialised shortcut output would be, and never written.
+ *   mask (nullable; uint8 [M, C / 8]): bit k of byte (row, v) = (y[row, 8v + k] > 0), taken from the bf16 value of
+ *   y as stored.  Write it when a backward follows.  Two launches (three with a shortcut BN).
+ * moco_bn_add_relu_bwd: g = dy masked by `mask`.  dbeta = sum g, dgamma = sum g * x^, dx as moco_bn_bwd.  Without a
+ *   shortcut BN, dresidual = g (nullable).  With one, the shortcut BN's backward runs in the same two passes on
+ *   the same g: its dbeta = sum g, dgamma = sum g * residual^, and dresidual is its input gradient (required).
+ *   Two launches.
+ * x, residual, y, dy, dx, dresidual: bf16 [M, C] row-major, 16-byte aligned, C a power of two in [64, 2048];
+ * workspace as for moco_bn_fwd_train (moco_bn_workspace_bytes() covers the three per-channel sums).
+ * ---------------------------------------------------------------------- */
+typedef struct moco_bn_layer {
+    const float* gamma;
+    const float* beta;
+    float* running_mean;
+    float* running_var;
+    long long* num_batches_tracked;
+    float momentum;
+    float eps;
+    float* save_mean;
+    float* save_invstd;
+    float* dgamma;
+    float* dbeta;
+} moco_bn_layer;
+
+int moco_bn_add_relu_fwd_train(const void* x, const void* residual, void* y, void* mask_or_null, long long M, int C,
+                               const moco_bn_layer* bn, const moco_bn_layer* shortcut_or_null,
+                               void* workspace, size_t workspace_bytes, void* stream);
+int moco_bn_add_relu_bwd(const void* dy, const void* x, const void* residual, const void* mask, long long M, int C,
+                         const moco_bn_layer* bn, const moco_bn_layer* shortcut_or_null, void* dx,
+                         void* dresidual_or_null, void* workspace, size_t workspace_bytes, void* stream);
+
+/* The stem's BatchNorm + ReLU followed by its 3x3 / stride 2 / pad 1 max pooling, without writing the BatchNorm's
+ * output: bit-identical to moco_bn_fwd_train (relu = 1, no residual) + moco_maxpool3x3s2_fwd.  The statistics pass,
+ * then one pass that applies BatchNorm + ReLU to every tap (rounded to bf16 as the BatchNorm's own pass stores it)
+ * and takes the max by torch's rule.  Two launches.
+ * x: bf16 [N, H, W, C] (NHWC storage), the BatchNorm's input, C a power of two in [64, 2048]; y, taps: the pooled
+ * output and the winning tap bytes as moco_maxpool3x3s2_fwd defines them; workspace as for moco_bn_fwd_train.
+ * The backward is moco_maxpool3x3s2_bwd followed by moco_bn_bwd (relu = 1, has_residual = 0), which recomputes the
+ * ReLU mask from x. */
+int moco_bn_relu_maxpool_fwd_train(const void* x, void* y, void* taps_u8, int N, int H, int W, int C,
+                                   const moco_bn_layer* bn, void* workspace, size_t workspace_bytes, void* stream);
+
 /* The same input pass (crop of the [N, C_total >= 3, H, W] batch, optional row permutation, cast to bf16) written in
  * the layout of a space-to-depth stem: dst = bf16 [N, H/2 + 3, W/2 + 3, 16] with
  *     dst[n, R, Q, (b * 2 + d) * 3 + c] = src[rows[n], c, 2 (R - 2) + b, 2 (Q - 2) + d]   (0 outside; channels 12..15 = 0)

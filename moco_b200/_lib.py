@@ -19,6 +19,15 @@ NCE_TWO_PASS, NCE_ONE_PASS = 512, 1024
 ONE_PASS_MAX_INV_T = 25.0          # MOCO_ONE_PASS_MAX_INV_T (include/moco_b200.h)
 GATHER_AUTO, GATHER_LDG = 0, 1
 
+
+
+class BnLayer(ctypes.Structure):
+    """moco_bn_layer (include/moco_b200.h): one BatchNorm's device pointers and hyper-parameters."""
+    _fields_ = [("gamma", c_void_p), ("beta", c_void_p), ("running_mean", c_void_p), ("running_var", c_void_p),
+                ("num_batches_tracked", c_void_p), ("momentum", c_float), ("eps", c_float),
+                ("save_mean", c_void_p), ("save_invstd", c_void_p), ("dgamma", c_void_p), ("dbeta", c_void_p)]
+
+
 # every symbol include/moco_b200.h declares: name -> (restype, argtypes)
 SIGNATURES = {
     "moco_abi_version": (c_int, []),
@@ -58,6 +67,12 @@ SIGNATURES = {
                                   c_void_p, c_float, c_float, c_int, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "moco_bn_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_void_p, c_void_p,
                             c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "moco_bn_add_relu_fwd_train": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, POINTER(BnLayer),
+                                           POINTER(BnLayer), c_void_p, c_size_t, c_void_p]),
+    "moco_bn_add_relu_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, POINTER(BnLayer),
+                                     POINTER(BnLayer), c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "moco_bn_relu_maxpool_fwd_train": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
+                                               POINTER(BnLayer), c_void_p, c_size_t, c_void_p]),
     "moco_crop_to_nhwc_bf16": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_int, c_int, c_void_p]),
     "moco_shuffle_gather": (c_int, [POINTER(c_void_p), c_int, c_int, c_void_p, c_int, c_size_t, c_void_p, c_int, c_void_p]),
     "moco_shuffle_gather_sync": (c_int, [POINTER(c_void_p), POINTER(c_void_p), c_int, c_int, c_uint32, c_int, c_void_p, c_int,
@@ -112,7 +127,7 @@ class _Counting:
 
     _PER_CALL = {"moco_nce_shard_stats": 3, "moco_nce_shard_merge": 1, "moco_nce_shard_dq": 2,
                  "moco_nce_shard_dq_finish": 1, "moco_nce_shard_dq_finish_peers": 1, "moco_queue_enqueue_shard": 1, "moco_queue_enqueue": 1, "moco_f32_to_bf16": 1, "moco_shuffle_gather": 1, "moco_shuffle_gather_sync": 1, "moco_crop_gather_nhwc_bf16": 1,
-                 "moco_ema_update": 1, "moco_crop_to_nhwc_bf16": 1, "moco_bn_fwd_train": 2, "moco_bn_bwd": 2, "moco_crop_s2d_bf16": 1, "moco_maxpool3x3s2_fwd": 1, "moco_maxpool3x3s2_bwd": 1,
+                 "moco_ema_update": 1, "moco_crop_to_nhwc_bf16": 1, "moco_bn_fwd_train": 2, "moco_bn_bwd": 2, "moco_bn_add_relu_bwd": 2, "moco_bn_relu_maxpool_fwd_train": 2, "moco_crop_s2d_bf16": 1, "moco_maxpool3x3s2_fwd": 1, "moco_maxpool3x3s2_bwd": 1,
                  "moco_signal_barrier": 1, "moco_nce_bwd_dense": 1}
 
     def __init__(self, lib):
@@ -125,6 +140,8 @@ class _Counting:
                 setattr(self, name, self._wrap_step(fn))
             elif name == "moco_nce_shard_dq":      # one-pass finish: dq_reduce only; two-pass: dq kernel + dq_reduce
                 setattr(self, name, self._wrap_flags(fn, 11))
+            elif name == "moco_bn_add_relu_fwd_train":  # + the shortcut BN's statistics pass
+                setattr(self, name, self._wrap_count(fn, lambda a: 3 if a[7] is not None else 2))
             elif name in self._PER_CALL:
                 setattr(self, name, self._wrap(fn, self._PER_CALL[name]))
             else:
@@ -137,6 +154,16 @@ class _Counting:
             rc = fn(*a)
             if rc == 0:
                 launches += n
+            return rc
+        return call
+
+    @staticmethod
+    def _wrap_count(fn, count):
+        def call(*a):
+            global launches
+            rc = fn(*a)
+            if rc == 0:
+                launches += count(a)
             return rc
         return call
 

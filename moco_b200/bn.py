@@ -5,6 +5,13 @@ The reference's encoders apply ``nn.BatchNorm2d`` -> [``out += residual``] -> [`
 batch statistics, and left to ATen's channels_last kernels they take most of the GPU time of a step.  :class:`BatchNormAct2d` is an ``nn.BatchNorm2d`` (same parameters,
 buffers and ``state_dict`` keys, same running-statistics updates) whose training-mode forward / backward on CUDA
 bf16 channels_last activations are two launches each of ``csrc/bn_nhwc.cu`` (``moco_bn_fwd_train`` / ``moco_bn_bwd``).
+A block's residual BatchNorm, ``relu(bn(x) + r)``, runs ``moco_bn_add_relu_*`` instead: the forward writes the ReLU
+mask as bits for the backward rather than having it re-read ``y``, and in a downsample block (``forward(x, residual,
+shortcut_bn=...)``) the shortcut's BatchNorm runs inside the same passes, so neither its output nor the gradient
+between the two BatchNorms is ever written.  The stem's BatchNorm + ReLU and its max pool (``forward_maxpool``) run
+as ``moco_bn_relu_maxpool_fwd_train``: the pool applies the BatchNorm to each tap, so the stem's full-resolution
+activation is never written.
+The results are bit-identical to the separate calls.
 Everything else -- CPU tensors, eval mode, fp32 or NCHW activations, channel counts the kernels do not take -- runs
 ``nn.BatchNorm2d``'s own forward followed by the add and the ReLU, i.e. exactly what the reference does.
 """
@@ -112,6 +119,128 @@ class _BatchNormActFn(torch.autograd.Function):
         return dx, dgamma, dbeta, dres, None, None, None, None, None, None
 
 
+def _layer(weight, bias, mean, invstd, stats=None, dgamma=None, dbeta=None):
+    """moco_bn_layer of one BatchNorm: stats = (running_mean, running_var, num_batches_tracked, momentum, eps)."""
+    ptr = lambda t: t.data_ptr() if t is not None else None
+    rm, rv, nbt, momentum, eps = stats if stats is not None else (None, None, None, 0.0, 0.0)
+    return _lib.BnLayer(ptr(weight), ptr(bias), ptr(rm), ptr(rv), ptr(nbt), float(momentum), float(eps), ptr(mean),
+                        ptr(invstd), ptr(dgamma), ptr(dbeta))
+
+
+class _BatchNormAddReluFn(torch.autograd.Function):
+    """y = relu(batch_norm_train(x) + r); r = residual, or with a shortcut BN r = bf16(shortcut_bn(residual)) where
+    residual is the shortcut convolution's raw output (a downsample block).  The backward reads the ReLU mask as bits
+    written by the forward instead of y; the shortcut BN's output and the gradient between the two BNs are never
+    materialised.  Same values as _BatchNormActFn (+ the shortcut BN's own pass)."""
+
+    @staticmethod
+    def forward(ctx, x, residual, weight, bias, sc_weight, sc_bias, stats, sc_stats, want_mask):
+        lib = _lib.load()
+        N, C, H, W = x.shape
+        M = N * H * W
+        y = torch.empty_like(x)
+        mask = torch.empty((M, C // 8), dtype=torch.uint8, device=x.device) if want_mask else None
+        f32 = lambda: torch.empty(C, dtype=torch.float32, device=x.device)
+        mean, invstd = f32(), f32()
+        bn = _layer(weight, bias, mean, invstd, stats)
+        sc, sc_mean, sc_invstd = None, None, None
+        if sc_weight is not None:
+            sc_mean, sc_invstd = f32(), f32()
+            sc = _layer(sc_weight, sc_bias, sc_mean, sc_invstd, sc_stats)
+        ws = _workspace(x.device)
+        # algorithmic bytes: statistics read x (+ the shortcut input); apply reads x and residual, writes y (+ mask bits)
+        nbytes = M * C * 2 * (4 + (sc is not None)) + (M * C // 8 if want_mask else 0)
+        code = _timed("bn_fwd", nbytes, lambda: lib.moco_bn_add_relu_fwd_train(
+            x.data_ptr(), residual.data_ptr(), y.data_ptr(), mask.data_ptr() if mask is not None else None, M, C, bn, sc,
+            ws.data_ptr(), ws.numel(), _lib.cur_stream()))
+        _lib.check(code, "moco_bn_add_relu_fwd_train")
+        ctx.save_for_backward(x, residual if sc is not None else None, mask, weight, mean, invstd, sc_weight, sc_mean,
+                              sc_invstd)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, residual, mask, weight, mean, invstd, sc_weight, sc_mean, sc_invstd = ctx.saved_tensors
+        if mask is None:
+            raise RuntimeError("moco_b200: BatchNormAct2d ran its forward without the ReLU mask (no input required grad)")
+        lib = _lib.load()
+        N, C, H, W = x.shape
+        M = N * H * W
+        if dy.dtype != torch.bfloat16:
+            dy = dy.to(torch.bfloat16)
+        dy = dy.contiguous(memory_format=torch.channels_last)
+        dx = torch.empty_like(x)
+        f32 = lambda: torch.empty(C, dtype=torch.float32, device=x.device)
+        dgamma, dbeta = f32(), f32()
+        bn = _layer(weight, None, mean, invstd, dgamma=dgamma, dbeta=dbeta)
+        sc, sc_dgamma, sc_dbeta = None, None, None
+        if sc_weight is not None:
+            sc_dgamma, sc_dbeta = f32(), f32()
+            sc = _layer(sc_weight, None, sc_mean, sc_invstd, dgamma=sc_dgamma, dbeta=sc_dbeta)
+            dres = torch.empty_like(x)
+        else:
+            dres = torch.empty_like(x) if ctx.needs_input_grad[1] else None
+        ws = _workspace(x.device)
+        # algorithmic bytes: reduce reads dy, x, mask (+ shortcut input); apply reads the same and writes dx (+ d residual)
+        nbytes = M * C * 2 * (5 + (dres is not None) + 2 * (sc is not None)) + 2 * (M * C // 8)
+        code = _timed("bn_bwd", nbytes, lambda: lib.moco_bn_add_relu_bwd(
+            dy.data_ptr(), x.data_ptr(), residual.data_ptr() if residual is not None else None, mask.data_ptr(), M, C,
+            bn, sc, dx.data_ptr(), dres.data_ptr() if dres is not None else None, ws.data_ptr(), ws.numel(),
+            _lib.cur_stream()))
+        _lib.check(code, "moco_bn_add_relu_bwd")
+        return dx, dres, dgamma, dbeta, sc_dgamma, sc_dbeta, None, None, None
+
+
+class _BatchNormReluMaxPoolFn(torch.autograd.Function):
+    """maxpool3x3s2(relu(batch_norm_train(x))) without writing the BatchNorm's output: the pool pass takes each tap
+    through the BatchNorm + ReLU.  The backward is the pool's backward followed by the BatchNorm's (mask from x).  Same
+    values as _BatchNormActFn followed by _MaxPool3x3s2Fn."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, stats):
+        lib = _lib.load()
+        N, C, H, W = x.shape
+        OH, OW = (H - 1) // 2 + 1, (W - 1) // 2 + 1
+        y = torch.empty((N, C, OH, OW), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
+        taps = torch.empty((N, OH, OW, C), dtype=torch.uint8, device=x.device)
+        mean = torch.empty(C, dtype=torch.float32, device=x.device)
+        invstd = torch.empty_like(mean)
+        bn = _layer(weight, bias, mean, invstd, stats)
+        ws = _workspace(x.device)
+        # algorithmic bytes: statistics read x; the pool pass reads x, writes y and the tap bytes
+        nbytes = N * H * W * C * 2 * 2 + N * OH * OW * C * 3
+        code = _timed("bn_fwd", nbytes, lambda: lib.moco_bn_relu_maxpool_fwd_train(
+            x.data_ptr(), y.data_ptr(), taps.data_ptr(), N, H, W, C, bn, ws.data_ptr(), ws.numel(), _lib.cur_stream()))
+        _lib.check(code, "moco_bn_relu_maxpool_fwd_train")
+        ctx.save_for_backward(x, taps, weight, bias, mean, invstd)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, taps, weight, bias, mean, invstd = ctx.saved_tensors
+        lib = _lib.load()
+        N, C, H, W = x.shape
+        if dy.dtype != torch.bfloat16:
+            dy = dy.to(torch.bfloat16)
+        dy = dy.contiguous(memory_format=torch.channels_last)
+        # Rebuilding the pool's input gradient inside the BatchNorm's two passes (a <= 4-window gather per element)
+        # measured slower than writing it once and streaming it: the pool's backward, then the BatchNorm's.
+        g = torch.empty_like(x)
+        _lib.check(lib.moco_maxpool3x3s2_bwd(dy.data_ptr(), taps.data_ptr(), g.data_ptr(), N, H, W, C, _lib.cur_stream()),
+                   "moco_maxpool3x3s2_bwd")
+        dx = torch.empty_like(x)
+        dgamma = torch.empty(C, dtype=torch.float32, device=x.device)
+        dbeta = torch.empty_like(dgamma)
+        ws = _workspace(x.device)
+        # algorithmic bytes: reduce reads g, x; apply reads g, x and writes dx
+        code = _timed("bn_bwd", N * H * W * C * 2 * 5, lambda: lib.moco_bn_bwd(
+            g.data_ptr(), x.data_ptr(), None, N * H * W, C, weight.data_ptr(), bias.data_ptr(), mean.data_ptr(),
+            invstd.data_ptr(), 1, 0, dx.data_ptr(), None, dgamma.data_ptr(), dbeta.data_ptr(), ws.data_ptr(),
+            ws.numel(), _lib.cur_stream()))
+        _lib.check(code, "moco_bn_bwd")
+        return dx, dgamma, dbeta, None
+
+
 class BatchNormAct2d(nn.BatchNorm2d):
     """``nn.BatchNorm2d`` + optional residual add + optional ReLU (``forward(x, residual=None)``)."""
 
@@ -128,8 +257,21 @@ class BatchNormAct2d(nn.BatchNorm2d):
                 and self.weight.dtype == torch.float32 and self.weight.is_cuda
                 and (self.running_mean is None or self.running_mean.dtype == torch.float32))
 
-    def forward(self, x, residual=None):
+    def _stats(self):
+        return (self.running_mean, self.running_var, self.num_batches_tracked if self.track_running_stats else None,
+                self.momentum, self.eps)
+
+    def forward(self, x, residual=None, shortcut_bn=None):
+        """``shortcut_bn``: a downsample block's shortcut BatchNorm (no ReLU); ``residual`` is then its input, the
+        shortcut convolution's raw output, and ``y = relu?(bn(x) + shortcut_bn(residual))``."""
+        if shortcut_bn is not None:
+            if (self.relu and not shortcut_bn.relu and self._fusable(x, residual)
+                    and shortcut_bn._fusable(residual, None)):
+                return self._add_relu(x, residual, shortcut_bn)
+            residual = shortcut_bn(residual)
         if self._fusable(x, residual):
+            if self.relu and residual is not None:
+                return self._add_relu(x, residual, None)
             return _BatchNormActFn.apply(x, self.weight, self.bias, residual, self.running_mean, self.running_var,
                                          self.num_batches_tracked if self.track_running_stats else None,
                                          self.momentum, self.eps, self.relu)
@@ -137,6 +279,20 @@ class BatchNormAct2d(nn.BatchNorm2d):
         if residual is not None:
             y = y + residual
         return F.relu(y, inplace=True) if self.relu else y
+
+    def forward_maxpool(self, x, pool):
+        """``pool(self(x))`` for a :class:`MaxPool3x3s2` ``pool`` (the stem): one pass applies the BatchNorm + ReLU to
+        every tap of the pool, so that the BatchNorm's output is never written."""
+        if self.relu and isinstance(pool, MaxPool3x3s2) and self._fusable(x, None):
+            return _BatchNormReluMaxPoolFn.apply(x, self.weight, self.bias, self._stats())
+        return pool(self(x))
+
+    def _add_relu(self, x, residual, sc):
+        params = (x, residual, self.weight, self.bias) + ((sc.weight, sc.bias) if sc is not None else ())
+        want_mask = torch.is_grad_enabled() and any(t.requires_grad for t in params)
+        return _BatchNormAddReluFn.apply(x, residual, self.weight, self.bias,
+                                         sc.weight if sc is not None else None, sc.bias if sc is not None else None,
+                                         self._stats(), sc._stats() if sc is not None else None, want_mask)
 
     def extra_repr(self):
         return super().extra_repr() + f", relu={self.relu}"

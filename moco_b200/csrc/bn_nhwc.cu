@@ -36,13 +36,14 @@ constexpr int kBnSlab = 64;                          // channels per reduction C
 constexpr int kBnLanes = kBnSlab / 8;                // 16-byte vectors per slab row
 constexpr int kBnRows = kBnThreads / kBnLanes;       // rows per pass
 constexpr int kBnMaxSlabs = 32;                      // C <= 2048
-constexpr int kBnPartial = 2 * kBnSlab;              // floats per CTA partial
+constexpr int kBnMaxPartial = 3 * kBnSlab;           // floats per CTA partial: up to three sums per channel
 // (16-byte loads in flight per thread and operand, resident CTAs per SM) of each kernel; every grid is one resident
 // wave (tools/bn_kernel_times.py times the variants over the layers of ResNet-50).
 constexpr int kBnStatsUnroll = 8, kBnStatsCtas = 2;
 constexpr int kBnApplyUnroll = 8, kBnApplyCtas = 2;
 constexpr int kBnBwdReduceUnroll = 4, kBnBwdReduceCtas = 2;
 constexpr int kBnBwdApplyUnroll = 2, kBnBwdApplyCtas = 3;
+constexpr int kBnBwdApplyScUnroll = 2, kBnBwdApplyScCtas = 2;   // with the shortcut BN: 48 coefficients per thread
 constexpr int kBnSms = 132;
 constexpr int kBnMaxCtas = kBnSms * 4;               // workspace sizing: no reduction grid is larger
 
@@ -64,36 +65,41 @@ __device__ __forceinline__ uint4 pack8(const float* f) {
     return u;
 }
 
-// Sum the 16 per-thread accumulators over the CTA's 32 row groups.  Returns, in threads j < 128, element j of the CTA
-// partial: j = v * 16 + k with v = 16-byte lane (8 channels), k < 8 the first sum, k >= 8 the second.
-__device__ __forceinline__ float slab_reduce(float (&acc)[16], float* red /*[8 * 128]*/) {
+// Sum the 8 * S per-thread accumulators (S per-channel sums of 8 channels) over the CTA's 32 row groups.  Returns, in
+// threads j < 64 * S, element j of the CTA partial: j = v * 8S + k with v = 16-byte lane (8 channels), k < 8 the first
+// sum, 8 <= k < 16 the second, 16 <= k < 24 the third.  Each element is added in the same order whatever S is.
+template <int S>
+__device__ __forceinline__ float slab_reduce(float (&acc)[8 * S], float* red /*[8 * 64S]*/) {
+    constexpr int P = S * kBnSlab;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
-    for (int k = 0; k < 16; ++k) {
+    for (int k = 0; k < 8 * S; ++k) {
         acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], 8);
         acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], 16);
     }
     if (lane < 8) {
 #pragma unroll
-        for (int k = 0; k < 16; ++k) red[warp * 128 + lane * 16 + k] = acc[k];
+        for (int k = 0; k < 8 * S; ++k) red[warp * P + lane * 8 * S + k] = acc[k];
     }
     __syncthreads();
     float t = 0.f;
-    if (threadIdx.x < 128) {
+    if (threadIdx.x < P) {
 #pragma unroll
-        for (int w = 0; w < kBnThreads / 32; ++w) t += red[w * 128 + threadIdx.x];
+        for (int w = 0; w < kBnThreads / 32; ++w) t += red[w * P + threadIdx.x];
     }
     return t;
 }
 
-// Publishes this CTA's partial, and in the last CTA of the slab to arrive returns true with the slab totals in
-// tot[128] (same element order as slab_reduce).  The R partials are added in a fixed order: warp w takes partials
-// w, w + 8, ... (lane l owns floats 4l .. 4l+3 of each, one coalesced 512-byte read per partial, 16 reads in flight),
-// then the 8 warps' sums are added in warp order.
+// Publishes this CTA's partial (64S floats), and in the last CTA of the slab to arrive returns true with the slab
+// totals in tot[64S] (same element order as slab_reduce).  The R partials are added in a fixed order: warp w takes
+// partials w, w + 8, ... (lane l owns floats 4l .. 4l+3 of each 128-float chunk, one coalesced 512-byte read per
+// partial and chunk, 16 reads in flight), then the 8 warps' sums are added in warp order.
+template <int S>
 __device__ __forceinline__ bool slab_finish(float part, float* partial, unsigned int* counter, int slab, int r, int R,
-                                            double* tot /*[8 * 128] shared*/, int* flag /*shared*/) {
-    float* mine = partial + ((size_t)slab * R + r) * kBnPartial;
-    if (threadIdx.x < kBnPartial) mine[threadIdx.x] = part;
+                                            double* tot /*[8 * 64S] shared*/, int* flag /*shared*/) {
+    constexpr int P = S * kBnSlab;
+    float* mine = partial + ((size_t)slab * R + r) * P;
+    if (threadIdx.x < P) mine[threadIdx.x] = part;
     __threadfence();
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -104,28 +110,30 @@ __device__ __forceinline__ bool slab_finish(float part, float* partial, unsigned
     if (!*flag) return false;
     __threadfence();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const float4* base = reinterpret_cast<const float4*>(partial + (size_t)slab * R * kBnPartial) + lane;
-    double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;
-    constexpr int kBatch = 16;
-    for (int q0 = warp; q0 < R; q0 += 8 * kBatch) {
-        float4 v[kBatch];
+    const float4* base = reinterpret_cast<const float4*>(partial + (size_t)slab * R * P);
+    for (int c4 = lane; c4 < P / 4; c4 += 32) {
+        double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;
+        constexpr int kBatch = 16;
+        for (int q0 = warp; q0 < R; q0 += 8 * kBatch) {
+            float4 v[kBatch];
 #pragma unroll
-        for (int t = 0; t < kBatch; ++t) {
-            const int q = q0 + 8 * t;
-            v[t] = (q < R) ? __ldcg(base + (size_t)q * (kBnPartial / 4)) : make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int t = 0; t < kBatch; ++t) {
+                const int q = q0 + 8 * t;
+                v[t] = (q < R) ? __ldcg(base + (size_t)q * (P / 4) + c4) : make_float4(0.f, 0.f, 0.f, 0.f);
+            }
+#pragma unroll
+            for (int t = 0; t < kBatch; ++t) { s0 += v[t].x; s1 += v[t].y; s2 += v[t].z; s3 += v[t].w; }
         }
-#pragma unroll
-        for (int t = 0; t < kBatch; ++t) { s0 += v[t].x; s1 += v[t].y; s2 += v[t].z; s3 += v[t].w; }
+        double* mine_tot = tot + warp * P + c4 * 4;
+        mine_tot[0] = s0; mine_tot[1] = s1; mine_tot[2] = s2; mine_tot[3] = s3;
     }
-    double* mine_tot = tot + warp * kBnPartial + lane * 4;
-    mine_tot[0] = s0; mine_tot[1] = s1; mine_tot[2] = s2; mine_tot[3] = s3;
     __syncthreads();
-    if (threadIdx.x < kBnPartial) {
+    if (threadIdx.x < P) {
         double t = 0.0;
 #pragma unroll
-        for (int w = 0; w < 8; ++w) t += tot[w * kBnPartial + threadIdx.x];
+        for (int w = 0; w < 8; ++w) t += tot[w * P + threadIdx.x];
         __syncwarp();
-        tot[threadIdx.x] = t;                        // warp w' < 4 overwrites only slots its own lanes read last
+        tot[threadIdx.x] = t;                        // only this thread reads slot threadIdx.x (w = 0 above)
     }
     if (threadIdx.x == 0) *counter = 0u;             // re-armed for the next launch on this stream
     __syncthreads();
@@ -149,8 +157,8 @@ struct BnStatsArgs {
 template <int kUnroll, int kCtas>
 __global__ void __launch_bounds__(kBnThreads, kCtas)
 bn_stats_kernel(const BnStatsArgs a) {
-    __shared__ float red[8 * 128];
-    __shared__ double tot[8 * kBnPartial];
+    __shared__ float red[8 * 2 * kBnSlab];
+    __shared__ double tot[8 * 2 * kBnSlab];
     __shared__ int flag;
     const int slab = blockIdx.x, r = blockIdx.y;
     const int v = threadIdx.x & (kBnLanes - 1), rl = threadIdx.x >> 3;
@@ -190,8 +198,8 @@ bn_stats_kernel(const BnStatsArgs a) {
             }
         }
     }
-    const float part = slab_reduce(acc, red);
-    if (!slab_finish(part, a.partial, a.counters + slab, slab, r, a.R, tot, &flag)) return;
+    const float part = slab_reduce<2>(acc, red);
+    if (!slab_finish<2>(part, a.partial, a.counters + slab, slab, r, a.R, tot, &flag)) return;
     if (threadIdx.x < kBnSlab) {
         const int c8 = threadIdx.x >> 3, k = threadIdx.x & 7;
         const int c = slab * kBnSlab + threadIdx.x;
@@ -215,27 +223,46 @@ bn_stats_kernel(const BnStatsArgs a) {
 
 struct BnApplyArgs {
     const uint4* x;
-    const uint4* res;                // nullable
+    const uint4* res;                // nullable; with kShortcut the shortcut convolution's raw output
     uint4* y;
+    uint8_t* mask;                   // nullable: bit k of byte j = (y[8j + k] > 0), the ReLU mask of the backward
     long long V;                     // M * C / 8
     int C, relu;
     const float* mean;
     const float* invstd;
     const float* gamma;
     const float* beta;
+    const float* mean2;              // kShortcut: the shortcut BN, applied to res and rounded to bf16 before the add
+    const float* invstd2;
+    const float* gamma2;
+    const float* beta2;
 };
 
-template <int kUnroll, int kCtas>
+// 8 mask bits of one vector of y, from the bf16 values as stored (a positive value that rounds to zero is off)
+__device__ __forceinline__ unsigned int relu_bits(const uint4& y) {
+    float r[8];
+    unpack8(y, r);
+    unsigned int b = 0u;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) b |= (r[k] > 0.f ? 1u : 0u) << k;
+    return b;
+}
+
+template <int kUnroll, int kCtas, bool kShortcut>
 __global__ void __launch_bounds__(kBnThreads, kCtas)
 bn_apply_kernel(const BnApplyArgs a) {
     const int lanes = a.C >> 3;                      // a power of two <= 256: this thread's channel group is fixed
     const int v = threadIdx.x & (lanes - 1);
-    float ca[8], cb[8];
+    float ca[8], cb[8], ca2[kShortcut ? 8 : 1], cb2[kShortcut ? 8 : 1];
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
         const int c = v * 8 + k;
         ca[k] = __ldg(a.gamma + c) * __ldg(a.invstd + c);
         cb[k] = fmaf(-__ldg(a.mean + c), ca[k], __ldg(a.beta + c));
+        if constexpr (kShortcut) {
+            ca2[k] = __ldg(a.gamma2 + c) * __ldg(a.invstd2 + c);
+            cb2[k] = fmaf(-__ldg(a.mean2 + c), ca2[k], __ldg(a.beta2 + c));
+        }
     }
     const long long stride = (long long)gridDim.x * kBnThreads;
     const bool has_res = a.res != nullptr;
@@ -258,25 +285,35 @@ bn_apply_kernel(const BnApplyArgs a) {
                 float f[8], g[8];
                 unpack8(u[t], f);
                 unpack8(w[t], g);
+                if constexpr (kShortcut) {
+                    // what the shortcut BN's own pass stores (its "+ residual" is +0.f) and the add reads back
+#pragma unroll
+                    for (int k = 0; k < 8; ++k)
+                        g[k] = __bfloat162float(__float2bfloat16_rn(__fadd_rn(fmaf(g[k], ca2[k], cb2[k]), 0.f)));
+                }
 #pragma unroll
                 for (int k = 0; k < 8; ++k) {
                     float z = fmaf(f[k], ca[k], cb[k]) + g[k];
                     if (a.relu) z = fmaxf(z, 0.f);
                     f[k] = z;
                 }
-                a.y[j] = pack8(f);
+                const uint4 out = pack8(f);
+                a.y[j] = out;
+                if (a.mask != nullptr) a.mask[j] = (uint8_t)relu_bits(out);
             }
         }
     }
 }
 
 // how the ReLU mask of the backward is obtained
-enum { kMaskNone = 0, kMaskFromY = 1, kMaskFromX = 2 };
+enum { kMaskNone = 0, kMaskFromY = 1, kMaskFromX = 2, kMaskFromBits = 3 };
 
 struct BnBwdReduceArgs {
     const uint4* dy;
     const uint4* x;
     const uint4* y;                  // kMaskFromY only
+    const uint8_t* mbits;            // kMaskFromBits only: the forward's mask bytes
+    const uint4* x2;                 // kShortcut: the shortcut BN's input
     long long M, passes, ppc;
     int C, R, mask;
     float* partial;
@@ -285,74 +322,101 @@ struct BnBwdReduceArgs {
     const float* invstd;
     const float* gamma;
     const float* beta;
+    const float* mean2;              // kShortcut
+    const float* invstd2;
     float* sum_dy;                   // = dbeta
     float* sum_dy_xhat;              // = dgamma
+    float* sum_dy2;                  // kShortcut: = the shortcut BN's dbeta (the same sum)
+    float* sum_dy_xhat2;             // kShortcut: = the shortcut BN's dgamma
 };
 
-template <int kUnroll, int kCtas>
+__device__ __forceinline__ bool mask_on(int mode, float y, unsigned int bits, int k, float x, float ca, float cb) {
+    if (mode == kMaskFromY) return y > 0.f;
+    if (mode == kMaskFromX) return fmaf(x, ca, cb) > 0.f;
+    if (mode == kMaskFromBits) return (bits >> k) & 1u;
+    return true;
+}
+
+// kShortcut: the block's bn3 and the shortcut BN of a downsample block, both fed by the same masked gradient g: a
+// third sum, g * (x2 - mean2), taken in the same row / slab plan and per-thread order as the shortcut's own reduction.
+template <int kUnroll, int kCtas, bool kShortcut>
 __global__ void __launch_bounds__(kBnThreads, kCtas)
 bn_bwd_reduce_kernel(const BnBwdReduceArgs a) {
-    __shared__ float red[8 * 128];
-    __shared__ double tot[8 * kBnPartial];
+    constexpr int S = kShortcut ? 3 : 2;
+    __shared__ float red[8 * S * kBnSlab];
+    __shared__ double tot[8 * S * kBnSlab];
     __shared__ int flag;
     const int slab = blockIdx.x, r = blockIdx.y;
     const int v = threadIdx.x & (kBnLanes - 1), rl = threadIdx.x >> 3;
     const int vec_per_row = a.C >> 3;
     const int colv = slab * kBnLanes + v;
-    float mu[8], ca[8], cb[8];                       // sum(g x^) = invstd * sum(g (x - mean)): invstd applied at the end
+    const int mode = kShortcut ? (int)kMaskFromBits : a.mask;      // a downsample block's bn3 always has its mask bits
+    float mu[8], ca[8], cb[8], mu2[kShortcut ? 8 : 1]; // sum(g x^) = invstd * sum(g (x - mean)): invstd applied at the end
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
         const int c = colv * 8 + k;
         mu[k] = __ldg(a.mean + c);
-        ca[k] = __ldg(a.gamma + c) * __ldg(a.invstd + c);
-        cb[k] = fmaf(-mu[k], ca[k], __ldg(a.beta + c));
+        ca[k] = cb[k] = 0.f;
+        if (mode == kMaskFromX) {
+            ca[k] = __ldg(a.gamma + c) * __ldg(a.invstd + c);
+            cb[k] = fmaf(-mu[k], ca[k], __ldg(a.beta + c));
+        }
+        if constexpr (kShortcut) mu2[k] = __ldg(a.mean2 + c);
     }
-    float acc[16];
+    float acc[8 * S];
 #pragma unroll
-    for (int k = 0; k < 16; ++k) acc[k] = 0.f;
+    for (int k = 0; k < 8 * S; ++k) acc[k] = 0.f;
     const long long p0 = (long long)r * a.ppc;
     const long long p1 = (p0 + a.ppc < a.passes) ? p0 + a.ppc : a.passes;
     for (long long p = p0; p < p1; p += kUnroll) {
-        uint4 ud[kUnroll], ux[kUnroll], uy[kUnroll];
+        uint4 ud[kUnroll], ux[kUnroll], uy[kUnroll], u2[kShortcut ? kUnroll : 1];
+        unsigned int mb[kUnroll];
         bool live[kUnroll];
 #pragma unroll
         for (int t = 0; t < kUnroll; ++t) {
             const long long row = (p + t) * kBnRows + rl;
             live[t] = (p + t < p1) && row < a.M;
             ud[t] = ux[t] = uy[t] = make_uint4(0u, 0u, 0u, 0u);
+            if constexpr (kShortcut) u2[t] = make_uint4(0u, 0u, 0u, 0u);
+            mb[t] = 0u;
             if (live[t]) {
                 const long long j = row * vec_per_row + colv;
                 ud[t] = __ldg(a.dy + j);
                 ux[t] = __ldg(a.x + j);
-                if (a.mask == kMaskFromY) uy[t] = __ldg(a.y + j);
+                if (mode == kMaskFromY) uy[t] = __ldg(a.y + j);
+                if (mode == kMaskFromBits) mb[t] = __ldg(a.mbits + j);
+                if constexpr (kShortcut) u2[t] = __ldg(a.x2 + j);
             }
         }
 #pragma unroll
         for (int t = 0; t < kUnroll; ++t) {
             if (live[t]) {
-                float d[8], f[8], yy[8];
+                float d[8], f[8], yy[8], f2[kShortcut ? 8 : 1];
                 unpack8(ud[t], d);
                 unpack8(ux[t], f);
                 unpack8(uy[t], yy);
+                if constexpr (kShortcut) unpack8(u2[t], f2);
 #pragma unroll
                 for (int k = 0; k < 8; ++k) {
-                    bool on = true;
-                    if (a.mask == kMaskFromY) on = yy[k] > 0.f;
-                    else if (a.mask == kMaskFromX) on = fmaf(f[k], ca[k], cb[k]) > 0.f;
-                    const float g = on ? d[k] : 0.f;
+                    const float g = mask_on(mode, yy[k], mb[t], k, f[k], ca[k], cb[k]) ? d[k] : 0.f;
                     acc[k] += g;
                     acc[8 + k] = fmaf(g, f[k] - mu[k], acc[8 + k]);
+                    if constexpr (kShortcut) acc[16 + k] = fmaf(g, f2[k] - mu2[k], acc[16 + k]);
                 }
             }
         }
     }
-    const float part = slab_reduce(acc, red);
-    if (!slab_finish(part, a.partial, a.counters + slab, slab, r, a.R, tot, &flag)) return;
+    const float part = slab_reduce<S>(acc, red);
+    if (!slab_finish<S>(part, a.partial, a.counters + slab, slab, r, a.R, tot, &flag)) return;
     if (threadIdx.x < kBnSlab) {
         const int c8 = threadIdx.x >> 3, k = threadIdx.x & 7;
         const int c = slab * kBnSlab + threadIdx.x;
-        a.sum_dy[c] = (float)tot[c8 * 16 + k];
-        a.sum_dy_xhat[c] = (float)(tot[c8 * 16 + 8 + k] * (double)a.invstd[c]);
+        a.sum_dy[c] = (float)tot[c8 * 8 * S + k];
+        a.sum_dy_xhat[c] = (float)(tot[c8 * 8 * S + 8 + k] * (double)a.invstd[c]);
+        if constexpr (kShortcut) {
+            a.sum_dy2[c] = (float)tot[c8 * 8 * S + k];
+            a.sum_dy_xhat2[c] = (float)(tot[c8 * 8 * S + 16 + k] * (double)a.invstd2[c]);
+        }
     }
 }
 
@@ -360,8 +424,11 @@ struct BnBwdApplyArgs {
     const uint4* dy;
     const uint4* x;
     const uint4* y;                  // kMaskFromY only
+    const uint8_t* mbits;            // kMaskFromBits only
+    const uint4* x2;                 // kShortcut: the shortcut BN's input
     uint4* dx;
     uint4* dres;                     // nullable: the masked gradient, for the residual branch
+    uint4* dx2;                      // kShortcut: the shortcut BN's input gradient
     long long V;
     int C, mask;
     float inv_m;
@@ -371,39 +438,58 @@ struct BnBwdApplyArgs {
     const float* beta;
     const float* sum_dy;
     const float* sum_dy_xhat;
+    const float* mean2;              // kShortcut
+    const float* invstd2;
+    const float* gamma2;
+    const float* sum_dy_xhat2;
 };
 
-template <int kUnroll, int kCtas>
+// dx = k1 * (g - m1 - x^ * m2),  k1 = gamma * invstd, m1 = sum(g) / M, m2 = sum(g x^) / M, x^ = (x - mean) * invstd
+//    = cA * g + cB * x + cD
+__device__ __forceinline__ void bwd_coefs(float gamma, float mu, float is, float sum_dy, float sum_dy_xhat, float inv_m,
+                                          float& cA, float& cB, float& cD) {
+    const float k1 = gamma * is;
+    const float m1 = sum_dy * inv_m, m2 = sum_dy_xhat * inv_m;
+    cA = k1;
+    cB = -k1 * m2 * is;
+    cD = fmaf(-cB, mu, -k1 * m1);
+}
+
+template <int kUnroll, int kCtas, bool kShortcut>
 __global__ void __launch_bounds__(kBnThreads, kCtas)
 bn_bwd_apply_kernel(const BnBwdApplyArgs a) {
     const int lanes = a.C >> 3;
     const int v = threadIdx.x & (lanes - 1);
-    // dx = k1 * (g - m1 - x^ * m2),  k1 = gamma * invstd, m1 = sum(g) / M, m2 = sum(g x^) / M, x^ = (x - mean) * invstd
-    //    = cA * g + cB * x + cD
-    float cA[8], cB[8], cD[8], ca[8], cb[8];
+    const int mode = kShortcut ? (int)kMaskFromBits : a.mask;
+    constexpr int K2 = kShortcut ? 8 : 1;
+    float cA[8], cB[8], cD[8], ca[8], cb[8], cA2[K2], cB2[K2], cD2[K2];
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
         const int c = v * 8 + k;
         const float mu = __ldg(a.mean + c), is = __ldg(a.invstd + c);
-        const float k1 = __ldg(a.gamma + c) * is;
-        const float m1 = __ldg(a.sum_dy + c) * a.inv_m, m2 = __ldg(a.sum_dy_xhat + c) * a.inv_m;
-        cA[k] = k1;
-        cB[k] = -k1 * m2 * is;
-        cD[k] = fmaf(-cB[k], mu, -k1 * m1);
-        ca[k] = k1;
-        cb[k] = fmaf(-mu, k1, __ldg(a.beta + c));
+        bwd_coefs(__ldg(a.gamma + c), mu, is, __ldg(a.sum_dy + c), __ldg(a.sum_dy_xhat + c), a.inv_m, cA[k], cB[k], cD[k]);
+        ca[k] = cA[k];
+        cb[k] = mode == kMaskFromX ? fmaf(-mu, cA[k], __ldg(a.beta + c)) : 0.f;
+        if constexpr (kShortcut)
+            bwd_coefs(__ldg(a.gamma2 + c), __ldg(a.mean2 + c), __ldg(a.invstd2 + c), __ldg(a.sum_dy + c),
+                      __ldg(a.sum_dy_xhat2 + c), a.inv_m, cA2[k], cB2[k], cD2[k]);
     }
     const long long stride = (long long)gridDim.x * kBnThreads;
     for (long long i = (long long)blockIdx.x * kBnThreads + threadIdx.x; i < a.V; i += stride * kUnroll) {
-        uint4 ud[kUnroll], ux[kUnroll], uy[kUnroll];
+        uint4 ud[kUnroll], ux[kUnroll], uy[kUnroll], u2[kShortcut ? kUnroll : 1];
+        unsigned int mb[kUnroll];
 #pragma unroll
         for (int t = 0; t < kUnroll; ++t) {
             const long long j = i + t * stride;
             ud[t] = ux[t] = uy[t] = make_uint4(0u, 0u, 0u, 0u);
+            if constexpr (kShortcut) u2[t] = make_uint4(0u, 0u, 0u, 0u);
+            mb[t] = 0u;
             if (j < a.V) {
                 ud[t] = __ldg(a.dy + j);
                 ux[t] = __ldg(a.x + j);
-                if (a.mask == kMaskFromY) uy[t] = __ldg(a.y + j);
+                if (mode == kMaskFromY) uy[t] = __ldg(a.y + j);
+                if (mode == kMaskFromBits) mb[t] = __ldg(a.mbits + j);
+                if constexpr (kShortcut) u2[t] = __ldg(a.x2 + j);
             }
         }
 #pragma unroll
@@ -416,15 +502,19 @@ bn_bwd_apply_kernel(const BnBwdApplyArgs a) {
                 unpack8(uy[t], yy);
 #pragma unroll
                 for (int k = 0; k < 8; ++k) {
-                    bool on = true;
-                    if (a.mask == kMaskFromY) on = yy[k] > 0.f;
-                    else if (a.mask == kMaskFromX) on = fmaf(f[k], ca[k], cb[k]) > 0.f;
-                    const float g = on ? d[k] : 0.f;
+                    const float g = mask_on(mode, yy[k], mb[t], k, f[k], ca[k], cb[k]) ? d[k] : 0.f;
                     d[k] = g;
                     o[k] = fmaf(cA[k], g, fmaf(cB[k], f[k], cD[k]));
                 }
                 a.dx[j] = pack8(o);
-                if (a.dres != nullptr) a.dres[j] = pack8(d);
+                if constexpr (kShortcut) {
+                    unpack8(u2[t], f);
+#pragma unroll
+                    for (int k = 0; k < 8; ++k) o[k] = fmaf(cA2[k], d[k], fmaf(cB2[k], f[k], cD2[k]));
+                    a.dx2[j] = pack8(o);
+                } else if (a.dres != nullptr) {
+                    a.dres[j] = pack8(d);
+                }
             }
         }
     }
@@ -432,7 +522,7 @@ bn_bwd_apply_kernel(const BnBwdApplyArgs a) {
 
 // ---- host side ------------------------------------------------------------------------------------------------------
 
-size_t bn_workspace_bytes() { return 256 + (size_t)kBnMaxCtas * kBnPartial * sizeof(float); }
+size_t bn_workspace_bytes() { return 256 + (size_t)kBnMaxCtas * kBnMaxPartial * sizeof(float); }
 
 static bool bn_shape_ok(long long M, int C) {
     if (M < 1 || C < kBnSlab || C > kBnSlab * kBnMaxSlabs) return false;
@@ -465,27 +555,26 @@ static cudaError_t run_stats(BnStatsArgs& s, cudaStream_t stream) {
     bn_stats_kernel<U, CT><<<dim3(s.C / kBnSlab, s.R), kBnThreads, 0, stream>>>(s);
     return cudaGetLastError();
 }
-template <int U, int CT>
+template <int U, int CT, bool SC>
 static cudaError_t run_apply(BnApplyArgs& p, cudaStream_t stream) {
-    bn_apply_kernel<U, CT><<<bn_apply_grid(p.V, U, CT), kBnThreads, 0, stream>>>(p);
+    bn_apply_kernel<U, CT, SC><<<bn_apply_grid(p.V, U, CT), kBnThreads, 0, stream>>>(p);
     return cudaGetLastError();
 }
-template <int U, int CT>
+template <int U, int CT, bool SC>
 static cudaError_t run_bwd_reduce(BnBwdReduceArgs& s, cudaStream_t stream) {
     bn_reduce_plan(s.M, s.C, U, CT, &s.passes, &s.ppc, &s.R);
-    bn_bwd_reduce_kernel<U, CT><<<dim3(s.C / kBnSlab, s.R), kBnThreads, 0, stream>>>(s);
+    bn_bwd_reduce_kernel<U, CT, SC><<<dim3(s.C / kBnSlab, s.R), kBnThreads, 0, stream>>>(s);
     return cudaGetLastError();
 }
-template <int U, int CT>
+template <int U, int CT, bool SC>
 static cudaError_t run_bwd_apply(BnBwdApplyArgs& p, cudaStream_t stream) {
-    bn_bwd_apply_kernel<U, CT><<<bn_apply_grid(p.V, U, CT), kBnThreads, 0, stream>>>(p);
+    bn_bwd_apply_kernel<U, CT, SC><<<bn_apply_grid(p.V, U, CT), kBnThreads, 0, stream>>>(p);
     return cudaGetLastError();
 }
 
-cudaError_t launch_bn_fwd_train(const void* x, const void* res, void* y, long long M, int C, const float* gamma,
-                                const float* beta, float* running_mean, float* running_var, long long* nbt, float momentum,
-                                float eps, int relu, float* save_mean, float* save_invstd, void* ws, cudaStream_t stream) {
-    if (!bn_shape_ok(M, C)) return cudaErrorNotSupported;
+static cudaError_t stats_pass(const void* x, long long M, int C, float* running_mean, float* running_var, long long* nbt,
+                              float momentum, float eps, float* save_mean, float* save_invstd, void* ws,
+                              cudaStream_t stream) {
     BnStatsArgs s{};
     s.x = static_cast<const uint4*>(x);
     s.M = M; s.C = C;
@@ -494,13 +583,20 @@ cudaError_t launch_bn_fwd_train(const void* x, const void* res, void* y, long lo
     s.partial = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 256);
     s.mean = save_mean; s.invstd = save_invstd;
     s.running_mean = running_mean; s.running_var = running_var; s.num_batches_tracked = nbt;
-    cudaError_t e = run_stats<kBnStatsUnroll, kBnStatsCtas>(s, stream);
+    return run_stats<kBnStatsUnroll, kBnStatsCtas>(s, stream);
+}
+
+cudaError_t launch_bn_fwd_train(const void* x, const void* res, void* y, long long M, int C, const float* gamma,
+                                const float* beta, float* running_mean, float* running_var, long long* nbt, float momentum,
+                                float eps, int relu, float* save_mean, float* save_invstd, void* ws, cudaStream_t stream) {
+    if (!bn_shape_ok(M, C)) return cudaErrorNotSupported;
+    cudaError_t e = stats_pass(x, M, C, running_mean, running_var, nbt, momentum, eps, save_mean, save_invstd, ws, stream);
     if (e != cudaSuccess) return e;
     BnApplyArgs p{};
     p.x = static_cast<const uint4*>(x); p.res = static_cast<const uint4*>(res); p.y = static_cast<uint4*>(y);
     p.V = M * (C >> 3); p.C = C; p.relu = relu;
     p.mean = save_mean; p.invstd = save_invstd; p.gamma = gamma; p.beta = beta;
-    return run_apply<kBnApplyUnroll, kBnApplyCtas>(p, stream);
+    return run_apply<kBnApplyUnroll, kBnApplyCtas, false>(p, stream);
 }
 
 cudaError_t launch_bn_bwd(const void* dy, const void* x, const void* y, long long M, int C, const float* gamma,
@@ -516,14 +612,77 @@ cudaError_t launch_bn_bwd(const void* dy, const void* x, const void* y, long lon
     s.partial = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 256);
     s.mean = save_mean; s.invstd = save_invstd; s.gamma = gamma; s.beta = beta;
     s.sum_dy = dbeta; s.sum_dy_xhat = dgamma;
-    cudaError_t e = run_bwd_reduce<kBnBwdReduceUnroll, kBnBwdReduceCtas>(s, stream);
+    cudaError_t e = run_bwd_reduce<kBnBwdReduceUnroll, kBnBwdReduceCtas, false>(s, stream);
     if (e != cudaSuccess) return e;
     BnBwdApplyArgs p{};
     p.dy = s.dy; p.x = s.x; p.y = s.y; p.dx = static_cast<uint4*>(dx); p.dres = static_cast<uint4*>(dres);
     p.V = M * (C >> 3); p.C = C; p.mask = mask; p.inv_m = (float)(1.0 / (double)M);
     p.mean = save_mean; p.invstd = save_invstd; p.gamma = gamma; p.beta = beta;
     p.sum_dy = dbeta; p.sum_dy_xhat = dgamma;
-    return run_bwd_apply<kBnBwdApplyUnroll, kBnBwdApplyCtas>(p, stream);
+    return run_bwd_apply<kBnBwdApplyUnroll, kBnBwdApplyCtas, false>(p, stream);
+}
+
+cudaError_t launch_bn_add_relu_fwd(const void* x, const void* res, void* y, void* mask, long long M, int C,
+                                   const BnLayer& bn, const BnLayer* sc, void* ws, cudaStream_t stream) {
+    if (!bn_shape_ok(M, C)) return cudaErrorNotSupported;
+    cudaError_t e = stats_pass(x, M, C, bn.running_mean, bn.running_var, bn.num_batches_tracked, bn.momentum, bn.eps,
+                               bn.save_mean, bn.save_invstd, ws, stream);
+    if (e == cudaSuccess && sc != nullptr)
+        e = stats_pass(res, M, C, sc->running_mean, sc->running_var, sc->num_batches_tracked, sc->momentum, sc->eps,
+                       sc->save_mean, sc->save_invstd, ws, stream);
+    if (e != cudaSuccess) return e;
+    BnApplyArgs p{};
+    p.x = static_cast<const uint4*>(x); p.res = static_cast<const uint4*>(res); p.y = static_cast<uint4*>(y);
+    p.mask = static_cast<uint8_t*>(mask);
+    p.V = M * (C >> 3); p.C = C; p.relu = 1;
+    p.mean = bn.save_mean; p.invstd = bn.save_invstd; p.gamma = bn.gamma; p.beta = bn.beta;
+    if (sc == nullptr) return run_apply<kBnApplyUnroll, kBnApplyCtas, false>(p, stream);
+    p.mean2 = sc->save_mean; p.invstd2 = sc->save_invstd; p.gamma2 = sc->gamma; p.beta2 = sc->beta;
+    return run_apply<kBnApplyUnroll, kBnApplyCtas, true>(p, stream);
+}
+
+cudaError_t launch_bn_add_relu_bwd(const void* dy, const void* x, const void* res, const void* mask, long long M, int C,
+                                   const BnLayer& bn, const BnLayer* sc, void* dx, void* dres, void* ws,
+                                   cudaStream_t stream) {
+    if (!bn_shape_ok(M, C)) return cudaErrorNotSupported;
+    BnBwdReduceArgs s{};
+    s.dy = static_cast<const uint4*>(dy); s.x = static_cast<const uint4*>(x);
+    s.mbits = static_cast<const uint8_t*>(mask);
+    s.M = M; s.C = C; s.mask = kMaskFromBits;
+    s.counters = static_cast<unsigned int*>(ws);
+    s.partial = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 256);
+    s.mean = bn.save_mean; s.invstd = bn.save_invstd; s.gamma = bn.gamma;
+    s.sum_dy = bn.dbeta; s.sum_dy_xhat = bn.dgamma;
+    BnBwdApplyArgs p{};
+    p.dy = s.dy; p.x = s.x; p.mbits = s.mbits; p.dx = static_cast<uint4*>(dx);
+    p.V = M * (C >> 3); p.C = C; p.mask = kMaskFromBits; p.inv_m = (float)(1.0 / (double)M);
+    p.mean = bn.save_mean; p.invstd = bn.save_invstd; p.gamma = bn.gamma;
+    p.sum_dy = bn.dbeta; p.sum_dy_xhat = bn.dgamma;
+    cudaError_t e;
+    if (sc == nullptr) {
+        p.dres = static_cast<uint4*>(dres);
+        e = run_bwd_reduce<kBnBwdReduceUnroll, kBnBwdReduceCtas, false>(s, stream);
+        if (e != cudaSuccess) return e;
+        return run_bwd_apply<kBnBwdApplyUnroll, kBnBwdApplyCtas, false>(p, stream);
+    }
+    s.x2 = static_cast<const uint4*>(res);
+    s.mean2 = sc->save_mean; s.invstd2 = sc->save_invstd;
+    s.sum_dy2 = sc->dbeta; s.sum_dy_xhat2 = sc->dgamma;
+    e = run_bwd_reduce<kBnBwdReduceUnroll, kBnBwdReduceCtas, true>(s, stream);
+    if (e != cudaSuccess) return e;
+    p.x2 = s.x2; p.dx2 = static_cast<uint4*>(dres);
+    p.mean2 = sc->save_mean; p.invstd2 = sc->save_invstd; p.gamma2 = sc->gamma; p.sum_dy_xhat2 = sc->dgamma;
+    return run_bwd_apply<kBnBwdApplyScUnroll, kBnBwdApplyScCtas, true>(p, stream);
+}
+
+cudaError_t launch_bn_relu_maxpool_fwd(const void* x, void* y, void* taps, int N, int H, int W, int C, const BnLayer& bn,
+                                       void* ws, cudaStream_t stream) {
+    const long long M = (long long)N * H * W;
+    if (N < 1 || H < 1 || W < 1 || !bn_shape_ok(M, C)) return cudaErrorNotSupported;
+    cudaError_t e = stats_pass(x, M, C, bn.running_mean, bn.running_var, bn.num_batches_tracked, bn.momentum, bn.eps,
+                               bn.save_mean, bn.save_invstd, ws, stream);
+    if (e != cudaSuccess) return e;
+    return launch_maxpool_fwd(x, y, taps, N, H, W, C, stream, bn.save_mean, bn.save_invstd, bn.gamma, bn.beta);
 }
 
 }  // namespace moco

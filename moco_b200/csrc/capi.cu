@@ -546,6 +546,77 @@ int moco_bn_bwd(const void* dy, const void* x, const void* y, long long M, int C
     return MOCO_OK;
 }
 
+static bool bn_layer_fwd_ok(const moco_bn_layer* b) {
+    return b && b->gamma && b->beta && b->save_mean && b->save_invstd &&
+           (b->running_mean == nullptr) == (b->running_var == nullptr) && b->eps > 0.f;
+}
+
+static bool bn_layer_bwd_ok(const moco_bn_layer* b) {
+    return b && b->gamma && b->save_mean && b->save_invstd && b->dgamma && b->dbeta;
+}
+
+int moco_bn_add_relu_fwd_train(const void* x, const void* residual, void* y, void* mask, long long M, int C,
+                               const moco_bn_layer* bn, const moco_bn_layer* shortcut, void* workspace,
+                               size_t workspace_bytes, void* stream_) {
+    g_err[0] = 0;
+    if (!x || !residual || !y || !workspace || !bn_layer_fwd_ok(bn) || (shortcut && !bn_layer_fwd_ok(shortcut)) ||
+        misaligned16(x) || misaligned16(residual) || misaligned16(y) || misaligned16(workspace) || x == y || residual == y) {
+        set_error("moco_bn_add_relu_fwd_train: bad argument (null / misaligned pointer, in-place, eps <= 0, "
+                  "one of running_mean / running_var)");
+        return MOCO_ERR_INVALID;
+    }
+    if (workspace_bytes < bn_workspace_bytes()) { set_error("moco_bn_add_relu_fwd_train: workspace too small"); return MOCO_ERR_WORKSPACE; }
+    cudaError_t e = launch_bn_add_relu_fwd(x, residual, y, mask, M, C, *bn, shortcut, workspace,
+                                           static_cast<cudaStream_t>(stream_));
+    if (e == cudaErrorNotSupported) {
+        set_error("moco_bn_add_relu_fwd_train: needs M >= 1 and C a power of two in [64, 2048] (M=%lld C=%d)", M, C);
+        return MOCO_ERR_UNSUPPORTED;
+    }
+    if (e != cudaSuccess) return cuda_fail("batch-norm forward kernels", e);
+    return MOCO_OK;
+}
+
+int moco_bn_add_relu_bwd(const void* dy, const void* x, const void* residual, const void* mask, long long M, int C,
+                         const moco_bn_layer* bn, const moco_bn_layer* shortcut, void* dx, void* dresidual,
+                         void* workspace, size_t workspace_bytes, void* stream_) {
+    g_err[0] = 0;
+    if (!dy || !x || !mask || !dx || !workspace || !bn_layer_bwd_ok(bn) ||
+        (shortcut && (!bn_layer_bwd_ok(shortcut) || !residual || !dresidual)) || misaligned16(dy) || misaligned16(x) ||
+        misaligned16(residual) || misaligned16(dx) || misaligned16(dresidual) || misaligned16(workspace)) {
+        set_error("moco_bn_add_relu_bwd: bad argument (null / misaligned pointer; residual and dresidual are required "
+                  "with a shortcut BN)");
+        return MOCO_ERR_INVALID;
+    }
+    if (workspace_bytes < bn_workspace_bytes()) { set_error("moco_bn_add_relu_bwd: workspace too small"); return MOCO_ERR_WORKSPACE; }
+    cudaError_t e = launch_bn_add_relu_bwd(dy, x, residual, mask, M, C, *bn, shortcut, dx, dresidual, workspace,
+                                           static_cast<cudaStream_t>(stream_));
+    if (e == cudaErrorNotSupported) {
+        set_error("moco_bn_add_relu_bwd: needs M >= 1 and C a power of two in [64, 2048] (M=%lld C=%d)", M, C);
+        return MOCO_ERR_UNSUPPORTED;
+    }
+    if (e != cudaSuccess) return cuda_fail("batch-norm backward kernels", e);
+    return MOCO_OK;
+}
+
+int moco_bn_relu_maxpool_fwd_train(const void* x, void* y, void* taps, int N, int H, int W, int C,
+                                   const moco_bn_layer* bn, void* workspace, size_t workspace_bytes, void* stream_) {
+    g_err[0] = 0;
+    if (!x || !y || !taps || !workspace || !bn_layer_fwd_ok(bn) || misaligned16(x) || misaligned16(y) ||
+        (reinterpret_cast<uintptr_t>(taps) & 7) || misaligned16(workspace)) {
+        set_error("moco_bn_relu_maxpool_fwd_train: bad argument (null / misaligned pointer, eps <= 0, "
+                  "one of running_mean / running_var)");
+        return MOCO_ERR_INVALID;
+    }
+    if (workspace_bytes < bn_workspace_bytes()) { set_error("moco_bn_relu_maxpool_fwd_train: workspace too small"); return MOCO_ERR_WORKSPACE; }
+    cudaError_t e = launch_bn_relu_maxpool_fwd(x, y, taps, N, H, W, C, *bn, workspace, static_cast<cudaStream_t>(stream_));
+    if (e == cudaErrorNotSupported) {
+        set_error("moco_bn_relu_maxpool_fwd_train: needs N, H, W >= 1 and C a power of two in [64, 2048] (C=%d)", C);
+        return MOCO_ERR_UNSUPPORTED;
+    }
+    if (e != cudaSuccess) return cuda_fail("batch-norm + max-pool forward kernels", e);
+    return MOCO_OK;
+}
+
 int moco_crop_to_nhwc_bf16(const void* src, int src_dtype, long long src_image_stride, void* dst, int N, int C, int HW,
                            void* stream_) {
     g_err[0] = 0;

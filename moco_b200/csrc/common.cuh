@@ -6,6 +6,8 @@
 #include <stdint.h>
 #include <stdlib.h>
 
+#include "../../include/moco_b200.h"
+
 namespace moco {
 
 constexpr int kMaxCtas = 160;          // upper bound on persistent CTAs (H100 SXM: 132 SMs)
@@ -91,7 +93,10 @@ cudaError_t launch_enqueue(__nv_bfloat16* queue_bf16, float* queue_f32, const vo
                            int n_all, int C, int64_t K, int64_t index, int64_t shard_row0, int64_t shard_rows,
                            cudaStream_t stream);
 cudaError_t launch_f32_to_bf16(const float* src, __nv_bfloat16* dst, size_t n, cudaStream_t stream);
-cudaError_t launch_maxpool_fwd(const void* x, void* y, void* idx, int N, int H, int W, int C, cudaStream_t stream);
+// bn_*: nullable; the stem's BatchNorm + ReLU applied to each tap (moco_bn_relu_maxpool_fwd_train)
+cudaError_t launch_maxpool_fwd(const void* x, void* y, void* idx, int N, int H, int W, int C, cudaStream_t stream,
+                               const float* bn_mean = nullptr, const float* bn_invstd = nullptr,
+                               const float* bn_gamma = nullptr, const float* bn_beta = nullptr);
 cudaError_t launch_maxpool_bwd(const void* dy, const void* idx, void* dx, int N, int H, int W, int C, cudaStream_t stream);
 cudaError_t launch_crop_to_s2d(const void* src, int src_dtype, long long img_stride, __nv_bfloat16* dst, int N, int H, int W,
                                cudaStream_t stream, const int64_t* src_rows);
@@ -102,6 +107,14 @@ cudaError_t launch_bn_fwd_train(const void* x, const void* res, void* y, long lo
 cudaError_t launch_bn_bwd(const void* dy, const void* x, const void* y, long long M, int C, const float* gamma,
                           const float* beta, const float* save_mean, const float* save_invstd, int relu, int has_residual,
                           void* dx, void* dres, float* dgamma, float* dbeta, void* ws, cudaStream_t stream);
+using BnLayer = moco_bn_layer;
+cudaError_t launch_bn_add_relu_fwd(const void* x, const void* res, void* y, void* mask, long long M, int C,
+                                   const BnLayer& bn, const BnLayer* sc, void* ws, cudaStream_t stream);
+cudaError_t launch_bn_add_relu_bwd(const void* dy, const void* x, const void* res, const void* mask, long long M, int C,
+                                   const BnLayer& bn, const BnLayer* sc, void* dx, void* dres, void* ws,
+                                   cudaStream_t stream);
+cudaError_t launch_bn_relu_maxpool_fwd(const void* x, void* y, void* taps, int N, int H, int W, int C, const BnLayer& bn,
+                                       void* ws, cudaStream_t stream);
 int ema_chunk_elems();
 cudaError_t launch_ema(const void* segs, const int* chunk_prefix, int n_segs, int n_chunks, float m,
                        float one_minus_m, cudaStream_t stream);

@@ -24,6 +24,12 @@ struct PoolArgs {
     uint2* idx;           // [N, OH, OW, C/8] x 8 tap bytes
     int N, H, W, OH, OW, lanes;
     long long total;      // vectors this launch produces
+    // forward, nullable: the stem's BatchNorm + ReLU applied to every tap (rounded to bf16 as its own pass stores it)
+    // before the max is taken -- the BatchNorm's output is never written
+    const float* mean;
+    const float* invstd;
+    const float* gamma;
+    const float* beta;
 };
 
 __device__ __forceinline__ void unpack8p(const uint4& u, float* f) {
@@ -46,6 +52,17 @@ maxpool3x3s2_fwd_kernel(const PoolArgs a) {
     p /= a.OW;
     const int oh = (int)(p % a.OH);
     const int n = (int)(p / a.OH);
+    const bool bn = a.gamma != nullptr;
+    float ca[8], cb[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        ca[k] = cb[k] = 0.f;
+        if (bn) {
+            const int c = cv * 8 + k;
+            ca[k] = __ldg(a.gamma + c) * __ldg(a.invstd + c);
+            cb[k] = fmaf(-__ldg(a.mean + c), ca[k], __ldg(a.beta + c));
+        }
+    }
     float m[8];
     unsigned int tap[8];
     bool first = true;
@@ -62,6 +79,11 @@ maxpool3x3s2_fwd_kernel(const PoolArgs a) {
             const uint4 u = __ldg(a.x + (((long long)n * a.H + ih) * a.W + iw) * a.lanes + cv);
             float f[8];
             unpack8p(u, f);
+            if (bn) {
+#pragma unroll
+                for (int k = 0; k < 8; ++k)       // bn_apply_kernel's relu(x * ca + cb + 0), rounded to bf16
+                    f[k] = __bfloat162float(__float2bfloat16_rn(fmaxf(__fadd_rn(fmaf(f[k], ca[k], cb[k]), 0.f), 0.f)));
+            }
             const unsigned int t = (unsigned int)(kh * 3 + kw);
 #pragma unroll
             for (int k = 0; k < 8; ++k) {
@@ -132,10 +154,12 @@ static bool pool_shape(int N, int H, int W, int C, PoolArgs* a) {
     return true;
 }
 
-cudaError_t launch_maxpool_fwd(const void* x, void* y, void* idx, int N, int H, int W, int C, cudaStream_t stream) {
+cudaError_t launch_maxpool_fwd(const void* x, void* y, void* idx, int N, int H, int W, int C, cudaStream_t stream,
+                               const float* bn_mean, const float* bn_invstd, const float* bn_gamma, const float* bn_beta) {
     PoolArgs a{};
     if (!pool_shape(N, H, W, C, &a)) return cudaErrorNotSupported;
     a.x = static_cast<const uint4*>(x); a.y = static_cast<uint4*>(y); a.idx = static_cast<uint2*>(idx);
+    a.mean = bn_mean; a.invstd = bn_invstd; a.gamma = bn_gamma; a.beta = bn_beta;
     a.total = (long long)N * a.OH * a.OW * a.lanes;
     const long long blocks = (a.total + kPoolThreads - 1) / kPoolThreads;
     if (blocks > 0x7fffffffLL) return cudaErrorNotSupported;

@@ -34,7 +34,9 @@ class _Basic(nn.Module):
 
     def forward(self, x):
         y = self.bn1(self.conv1(x))
-        return self.bn2(self.conv2(y), x if self.short is None else self.short(x))
+        if self.short is None:
+            return self.bn2(self.conv2(y), x)
+        return self.bn2(self.conv2(y), self.short[0](x), shortcut_bn=self.short[1])   # one BN group for both
 
 
 class _Bottleneck(nn.Module):
@@ -56,7 +58,9 @@ class _Bottleneck(nn.Module):
     def forward(self, x):
         y = self.bn1(self.conv1(x))
         y = self.bn2(self.conv2(y))
-        return self.bn3(self.conv3(y), x if self.short is None else self.short(x))
+        if self.short is None:
+            return self.bn3(self.conv3(y), x)
+        return self.bn3(self.conv3(y), self.short[0](x), shortcut_bn=self.short[1])   # one BN group for both
 
 
 class StemConv(nn.Conv2d):
@@ -110,7 +114,8 @@ class MoCoResNet(nn.Module):
                 nn.init.zeros_(m.bias)
 
     def forward(self, x):
-        x = self.layers(self.stem(x))
+        conv, bn, _, pool = self.stem                 # index 2 is the Identity placeholder
+        x = self.layers(bn.forward_maxpool(conv(x), pool))
         x = torch.flatten(F.adaptive_avg_pool2d(x, 1), 1)
         x = self.fc(x).float()
         if not self.l2norm:
