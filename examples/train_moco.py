@@ -28,7 +28,7 @@ def parse_args(argv=None):
     ap.add_argument("--weight-decay", type=float, default=1e-4)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--epoch", type=int, default=1, help="ShuffleBN seed (train.py:258 uses the epoch number)")
-    ap.add_argument("--resume", default="", help="checkpoint written by --save (or by the reference: same keys)")
+    ap.add_argument("--resume", default="", help="checkpoint written by --save or by the reference (either key naming)")
     ap.add_argument("--save", default="")
     ap.add_argument("--persist-index", action="store_true", help="keep the queue write position across resume")
     ap.add_argument("--fuse-normalize", action="store_true",
@@ -43,6 +43,7 @@ def main(argv=None):
     import torch
     import torch.distributed as dist
     from moco_b200 import encoders
+    from moco_b200.encoders import from_reference_state_dict
     from moco_b200.NCE import MemoryMoCo
     from moco_b200.train_step import MoCoStep
     from moco_b200.util import moment_update
@@ -66,8 +67,8 @@ def main(argv=None):
                           momentum=args.momentum, weight_decay=args.weight_decay)        # train.py:183-187
     if args.resume:
         ckpt = torch.load(args.resume, map_location="cpu")                               # train.py:157-166
-        model.load_state_dict(ckpt["model"])
-        model_ema.load_state_dict(ckpt["model_ema"])
+        model.load_state_dict(from_reference_state_dict(ckpt["model"]))
+        model_ema.load_state_dict(from_reference_state_dict(ckpt["model_ema"]))
         contrast.load_state_dict(ckpt["contrast"])
         opt.load_state_dict(ckpt["optimizer"])
     if world > 1:
@@ -86,7 +87,7 @@ def main(argv=None):
     if args.save and rank == 0:
         net = model.module if hasattr(model, "module") else model
         torch.save({"model": net.state_dict(), "model_ema": model_ema.state_dict(), "contrast": contrast.state_dict(),
-                    "optimizer": opt.state_dict()}, args.save)                          # train.py:141-150
+                    "optimizer": opt.state_dict(), "epoch": args.epoch}, args.save)     # train.py:141-150
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()

@@ -325,6 +325,42 @@ int moco_bn_add_relu_bwd(const void* dy, const void* x, const void* residual, co
 int moco_bn_relu_maxpool_fwd_train(const void* x, void* y, void* taps_u8, int N, int H, int W, int C,
                                    const moco_bn_layer* bn, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ------------------------------------------------------------------------
+ * Frozen (eval-mode) BatchNorm for the linear probe's encoder forward (the reference's eval.py runs the pretrained
+ * ResNet in eval mode): the same groups as above with the running statistics folded into two per-channel fp32
+ * vectors by the caller,
+ *     scale = gamma / sqrt(running_var + eps),   shift = beta - running_mean * scale,
+ * so there is no statistics pass and no backward.  One launch each, no workspace.
+ *
+ * Numerical contract (fp32, every operation rounded to nearest, NO fused multiply-add; it therefore differs from the
+ * training apply pass, which uses fmaf, and is reproduced exactly by separate fp32 torch ops):
+ *     z = (x * scale) + shift
+ *     z = z + r                                          when there is a residual
+ *     z = z > 0 ? z : 0                                  when relu
+ *     y = bf16_rn(z)
+ * with r = residual, or with a shortcut BN r = bf16_rn((residual * sc_scale) + sc_shift): residual is then the
+ * shortcut convolution's raw output, rounded as its materialised BatchNorm output would be, and never written.
+ * The average pool: feat[n, c] = (sum over p = 0 .. HW-1 of f32(y[n, p, c]), added in increasing p) / HW, with
+ * y the bf16-rounded value and one IEEE division.
+ *
+ * x, residual, y: bf16 [M, C] row-major (NHWC storage), 16-byte aligned, C a power of two in [64, 2048];
+ * scale, shift, sc_scale, sc_shift: fp32 [C]; sc_scale / sc_shift both or neither, and only with a residual.
+ *
+ * moco_bn_eval_act: y = relu?(bn(x) [+ r]), bf16 [M, C].
+ * moco_bn_relu_maxpool_eval: the stem, relu(bn(x)) (relu always on) applied to each tap of the 3x3 / stride 2 / pad 1
+ *   max pool of moco_maxpool3x3s2_fwd, x [N, H, W, C] -> y [N, OH, OW, C]; no tap bytes are written.
+ * moco_bn_eval_act_avgpool: the last block's group followed by the global average pool, x [N, HW, C] ->
+ *   feat fp32 [N, C] (16-byte aligned); the [N, HW, C] map is never written.
+ * ---------------------------------------------------------------------- */
+int moco_bn_eval_act(const void* x, const void* residual_or_null, void* y, long long M, int C, const float* scale,
+                     const float* shift, int relu, const float* sc_scale_or_null, const float* sc_shift_or_null,
+                     void* stream);
+int moco_bn_relu_maxpool_eval(const void* x, void* y, int N, int H, int W, int C, const float* scale,
+                              const float* shift, void* stream);
+int moco_bn_eval_act_avgpool(const void* x, const void* residual_or_null, float* feat_f32, int N, int HW, int C,
+                             const float* scale, const float* shift, int relu, const float* sc_scale_or_null,
+                             const float* sc_shift_or_null, void* stream);
+
 /* The same input pass (crop of the [N, C_total >= 3, H, W] batch, optional row permutation, cast to bf16) written in
  * the layout of a space-to-depth stem: dst = bf16 [N, H/2 + 3, W/2 + 3, 16] with
  *     dst[n, R, Q, (b * 2 + d) * 3 + c] = src[rows[n], c, 2 (R - 2) + b, 2 (Q - 2) + d]   (0 outside; channels 12..15 = 0)

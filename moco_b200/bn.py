@@ -12,8 +12,16 @@ between the two BatchNorms is ever written.  The stem's BatchNorm + ReLU and its
 as ``moco_bn_relu_maxpool_fwd_train``: the pool applies the BatchNorm to each tap, so the stem's full-resolution
 activation is never written.
 The results are bit-identical to the separate calls.
-Everything else -- CPU tensors, eval mode, fp32 or NCHW activations, channel counts the kernels do not take -- runs
-``nn.BatchNorm2d``'s own forward followed by the add and the ReLU, i.e. exactly what the reference does.
+A FROZEN module (``frozen = True``, set by :meth:`moco_b200.encoders.MoCoResNet.freeze`) in eval mode under
+``torch.no_grad()`` -- the linear probe's encoder -- runs the eval kernels instead: the running statistics are folded
+into a per-channel scale / shift (re-folded whenever the weights or statistics change), and one launch applies the
+BatchNorm, the add (a downsample block's shortcut BatchNorm included) and the ReLU (``moco_bn_eval_act``), or also
+the stem's max pool (``moco_bn_relu_maxpool_eval``) or the global average pool (``forward(..., avgpool=True)``,
+``moco_bn_eval_act_avgpool``).  Their arithmetic is the header's eval contract, which separate fp32 torch ops
+reproduce bit for bit.
+Everything else -- CPU tensors, eval mode of a module that is not frozen, fp32 or NCHW activations, channel counts the
+kernels do not take -- runs ``nn.BatchNorm2d``'s own forward followed by the add and the ReLU, i.e. exactly what the
+reference does.
 """
 from __future__ import annotations
 
@@ -247,6 +255,9 @@ class BatchNormAct2d(nn.BatchNorm2d):
     def __init__(self, num_features, relu=False, **kw):
         super().__init__(num_features, **kw)
         self.relu = bool(relu)
+        self.frozen = False             # MoCoResNet.freeze(): eval mode without grad runs the eval kernels
+        self._fold_key = None
+        self._fold = None
 
     def _fusable(self, x, residual):
         C = self.num_features
@@ -257,18 +268,75 @@ class BatchNormAct2d(nn.BatchNorm2d):
                 and self.weight.dtype == torch.float32 and self.weight.is_cuda
                 and (self.running_mean is None or self.running_mean.dtype == torch.float32))
 
+    def _eval_ok(self, x, residual):
+        """The frozen path: eval mode, grad mode off, running statistics, and activations the kernels take."""
+        C = self.num_features
+        return (_enabled and self.frozen and not self.training and not torch.is_grad_enabled() and self.affine
+                and self.track_running_stats and self.running_mean is not None
+                and _rows_ok(x) and (residual is None or _rows_ok(residual, x))
+                and 64 <= C <= 2048 and (C & (C - 1)) == 0 and x.shape[1] == C
+                and self.weight.dtype == torch.float32 and self.weight.is_cuda
+                and self.running_var.dtype == torch.float32)
+
+    def folded(self):
+        """(scale, shift) fp32 [C]: weight / sqrt(running_var + eps) and bias - running_mean * scale.  Cached, and
+        re-folded whenever the weight, the bias or a running buffer is replaced or modified in place through the
+        tensor itself (``load_state_dict``, ``copy_``, optimizer steps): the cache key is each tensor's storage and
+        version counter.  Writes through ``.data`` do not advance the version counter; call
+        ``MoCoResNet.freeze()`` again after them, which drops the cached coefficients."""
+        ts = (self.weight, self.bias, self.running_mean, self.running_var)
+        key = tuple((t.data_ptr(), t._version) for t in ts) + (self.eps,)
+        if key != self._fold_key:
+            with torch.no_grad():
+                scale = self.weight.float() / torch.sqrt(self.running_var.float() + self.eps)
+                shift = self.bias.float() - self.running_mean.float() * scale
+            self._fold, self._fold_key = (scale.contiguous(), shift.contiguous()), key
+        return self._fold
+
+    def _eval(self, x, residual, sc, avgpool):
+        lib = _lib.load()
+        N, C, H, W = x.shape
+        scale, shift = self.folded()
+        sc_scale, sc_shift = sc.folded() if sc is not None else (None, None)
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        # algorithmic bytes: reads x (+ residual), writes y (or the pooled fp32 features)
+        reads = N * H * W * C * 2 * (1 + (residual is not None))
+        if avgpool:
+            y = torch.empty((N, C), dtype=torch.float32, device=x.device)
+            code = _timed("bn_eval", reads + N * C * 4, lambda: lib.moco_bn_eval_act_avgpool(
+                x.data_ptr(), ptr(residual), y.data_ptr(), N, H * W, C, scale.data_ptr(), shift.data_ptr(),
+                int(self.relu), ptr(sc_scale), ptr(sc_shift), _lib.cur_stream()))
+            _lib.check(code, "moco_bn_eval_act_avgpool")
+            return y
+        y = torch.empty_like(x)
+        code = _timed("bn_eval", reads + N * H * W * C * 2, lambda: lib.moco_bn_eval_act(
+            x.data_ptr(), ptr(residual), y.data_ptr(), N * H * W, C, scale.data_ptr(), shift.data_ptr(),
+            int(self.relu), ptr(sc_scale), ptr(sc_shift), _lib.cur_stream()))
+        _lib.check(code, "moco_bn_eval_act")
+        return y
+
     def _stats(self):
         return (self.running_mean, self.running_var, self.num_batches_tracked if self.track_running_stats else None,
                 self.momentum, self.eps)
 
-    def forward(self, x, residual=None, shortcut_bn=None):
+    def forward(self, x, residual=None, shortcut_bn=None, avgpool=False):
         """``shortcut_bn``: a downsample block's shortcut BatchNorm (no ReLU); ``residual`` is then its input, the
-        shortcut convolution's raw output, and ``y = relu?(bn(x) + shortcut_bn(residual))``."""
+        shortcut convolution's raw output, and ``y = relu?(bn(x) + shortcut_bn(residual))``.  ``avgpool``: return
+        the global average pool of y, flattened to [N, C] (fp32 from the frozen path, y's dtype otherwise)."""
+        if avgpool:
+            if (shortcut_bn is None or not shortcut_bn.relu and shortcut_bn._eval_ok(residual, None)) \
+                    and self._eval_ok(x, residual):
+                return self._eval(x, residual, shortcut_bn, True)
+            return torch.flatten(F.adaptive_avg_pool2d(self.forward(x, residual, shortcut_bn), 1), 1)
         if shortcut_bn is not None:
+            if not shortcut_bn.relu and self._eval_ok(x, residual) and shortcut_bn._eval_ok(residual, None):
+                return self._eval(x, residual, shortcut_bn, False)
             if (self.relu and not shortcut_bn.relu and self._fusable(x, residual)
                     and shortcut_bn._fusable(residual, None)):
                 return self._add_relu(x, residual, shortcut_bn)
             residual = shortcut_bn(residual)
+        if self._eval_ok(x, residual):
+            return self._eval(x, residual, None, False)
         if self._fusable(x, residual):
             if self.relu and residual is not None:
                 return self._add_relu(x, residual, None)
@@ -283,6 +351,17 @@ class BatchNormAct2d(nn.BatchNorm2d):
     def forward_maxpool(self, x, pool):
         """``pool(self(x))`` for a :class:`MaxPool3x3s2` ``pool`` (the stem): one pass applies the BatchNorm + ReLU to
         every tap of the pool, so that the BatchNorm's output is never written."""
+        if self.relu and isinstance(pool, MaxPool3x3s2) and self._eval_ok(x, None):
+            lib = _lib.load()
+            N, C, H, W = x.shape
+            OH, OW = (H - 1) // 2 + 1, (W - 1) // 2 + 1
+            y = torch.empty((N, C, OH, OW), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
+            scale, shift = self.folded()
+            # algorithmic bytes: the pool pass reads x and writes y
+            code = _timed("bn_eval", N * H * W * C * 2 + N * OH * OW * C * 2, lambda: lib.moco_bn_relu_maxpool_eval(
+                x.data_ptr(), y.data_ptr(), N, H, W, C, scale.data_ptr(), shift.data_ptr(), _lib.cur_stream()))
+            _lib.check(code, "moco_bn_relu_maxpool_eval")
+            return y
         if self.relu and isinstance(pool, MaxPool3x3s2) and self._fusable(x, None):
             return _BatchNormReluMaxPoolFn.apply(x, self.weight, self.bias, self._stats())
         return pool(self(x))

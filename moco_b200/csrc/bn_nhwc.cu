@@ -520,6 +520,135 @@ bn_bwd_apply_kernel(const BnBwdApplyArgs a) {
     }
 }
 
+// ---- frozen (eval-mode) BatchNorm -----------------------------------------------------------------------------------
+// The per-channel scale / shift are folded by the caller from the running statistics; there is no statistics pass and
+// no backward.  Arithmetic is the header's numerical contract: no FMA contraction, so that separate fp32 torch ops
+// reproduce every bit.
+
+struct BnEvalArgs {
+    const uint4* x;
+    const uint4* res;                // nullable; with kShortcut the shortcut convolution's raw output
+    uint4* y;                        // element-wise pass
+    float* feat;                     // pooled pass: fp32 [N, C]
+    long long V;                     // element-wise: M * C / 8 vectors; pooled: N * C / 8 (one (image, vector) each)
+    int C, HW, relu;
+    const float* scale;
+    const float* shift;
+    const float* scale2;             // kShortcut
+    const float* shift2;
+};
+
+// z = relu?((x * s + t) [+ r]) in fp32, r = bf16((res * s2 + t2)) with a shortcut BN; returned unrounded
+template <bool kShortcut>
+__device__ __forceinline__ void bn_eval8(const uint4& ux, const uint4& ur, bool has_res, int relu, const float* s,
+                                         const float* t, const float* s2, const float* t2, float* z) {
+    float f[8], g[8];
+    unpack8(ux, f);
+    unpack8(ur, g);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        float v = __fadd_rn(__fmul_rn(f[k], s[k]), t[k]);
+        if (has_res) {
+            float r = g[k];
+            if constexpr (kShortcut) r = __bfloat162float(__float2bfloat16_rn(__fadd_rn(__fmul_rn(r, s2[k]), t2[k])));
+            v = __fadd_rn(v, r);
+        }
+        if (relu) v = v > 0.f ? v : 0.f;
+        z[k] = v;
+    }
+}
+
+template <bool kShortcut>
+__device__ __forceinline__ void bn_eval_coefs(const BnEvalArgs& a, int v, float* s, float* t, float* s2, float* t2) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const int c = v * 8 + k;
+        s[k] = __ldg(a.scale + c);
+        t[k] = __ldg(a.shift + c);
+        if constexpr (kShortcut) { s2[k] = __ldg(a.scale2 + c); t2[k] = __ldg(a.shift2 + c); }
+    }
+}
+
+template <bool kShortcut>
+__global__ void __launch_bounds__(kBnThreads, kBnApplyCtas)
+bn_eval_kernel(const BnEvalArgs a) {
+    const int v = threadIdx.x & ((a.C >> 3) - 1);    // fixed channel group, as in bn_apply_kernel
+    float s[8], t[8], s2[kShortcut ? 8 : 1], t2[kShortcut ? 8 : 1];
+    bn_eval_coefs<kShortcut>(a, v, s, t, s2, t2);
+    const long long stride = (long long)gridDim.x * kBnThreads;
+    const bool has_res = a.res != nullptr;
+    for (long long i = (long long)blockIdx.x * kBnThreads + threadIdx.x; i < a.V; i += stride * kBnApplyUnroll) {
+        uint4 u[kBnApplyUnroll], w[kBnApplyUnroll];
+#pragma unroll
+        for (int k = 0; k < kBnApplyUnroll; ++k) {
+            const long long j = i + k * stride;
+            u[k] = w[k] = make_uint4(0u, 0u, 0u, 0u);
+            if (j < a.V) {
+                u[k] = __ldg(a.x + j);
+                if (has_res) w[k] = __ldg(a.res + j);
+            }
+        }
+#pragma unroll
+        for (int k = 0; k < kBnApplyUnroll; ++k) {
+            const long long j = i + k * stride;
+            if (j < a.V) {
+                float z[8];
+                bn_eval8<kShortcut>(u[k], w[k], has_res, a.relu, s, t, s2, t2, z);
+                a.y[j] = pack8(z);
+            }
+        }
+    }
+}
+
+// The last block's BatchNorm (+ add + ReLU) followed by the global average pool: thread (n, v) walks the HW pixels of
+// image n in increasing order, adds the bf16-rounded outputs in fp32 and divides once.  The map is never written.
+// The pixel order is the contract, so the parallelism is N * C / 8 threads; 64-thread CTAs spread a small batch over
+// the SMs (N = 32 at C = 2048: 128 CTAs rather than 32 of 256 threads).
+constexpr int kBnPoolUnroll = 7;
+constexpr int kBnPoolThreads = 64;
+
+template <bool kShortcut>
+__global__ void __launch_bounds__(kBnPoolThreads, 8)   // 512 threads per SM: N = 256, C = 2048 is one wave
+bn_eval_avgpool_kernel(const BnEvalArgs a) {
+    const long long o = (long long)blockIdx.x * kBnPoolThreads + threadIdx.x;
+    if (o >= a.V) return;
+    const int lanes = a.C >> 3;
+    const int v = (int)(o & (lanes - 1));
+    const long long n = o / lanes;
+    float s[8], t[8], s2[kShortcut ? 8 : 1], t2[kShortcut ? 8 : 1];
+    bn_eval_coefs<kShortcut>(a, v, s, t, s2, t2);
+    const bool has_res = a.res != nullptr;
+    const long long base = n * a.HW * lanes + v;
+    float acc[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) acc[k] = 0.f;
+    for (int p0 = 0; p0 < a.HW; p0 += kBnPoolUnroll) {
+        uint4 u[kBnPoolUnroll], w[kBnPoolUnroll];
+#pragma unroll
+        for (int q = 0; q < kBnPoolUnroll; ++q) {
+            u[q] = w[q] = make_uint4(0u, 0u, 0u, 0u);
+            if (p0 + q < a.HW) {
+                const long long j = base + (long long)(p0 + q) * lanes;
+                u[q] = __ldg(a.x + j);
+                if (has_res) w[q] = __ldg(a.res + j);
+            }
+        }
+#pragma unroll
+        for (int q = 0; q < kBnPoolUnroll; ++q) {
+            if (p0 + q < a.HW) {
+                float z[8];
+                bn_eval8<kShortcut>(u[q], w[q], has_res, a.relu, s, t, s2, t2, z);
+#pragma unroll
+                for (int k = 0; k < 8; ++k) acc[k] = __fadd_rn(acc[k], __bfloat162float(__float2bfloat16_rn(z[k])));
+            }
+        }
+    }
+    const float hw = (float)a.HW;
+    float4* out = reinterpret_cast<float4*>(a.feat + n * a.C + v * 8);
+    out[0] = make_float4(__fdiv_rn(acc[0], hw), __fdiv_rn(acc[1], hw), __fdiv_rn(acc[2], hw), __fdiv_rn(acc[3], hw));
+    out[1] = make_float4(__fdiv_rn(acc[4], hw), __fdiv_rn(acc[5], hw), __fdiv_rn(acc[6], hw), __fdiv_rn(acc[7], hw));
+}
+
 // ---- host side ------------------------------------------------------------------------------------------------------
 
 size_t bn_workspace_bytes() { return 256 + (size_t)kBnMaxCtas * kBnMaxPartial * sizeof(float); }
@@ -683,6 +812,49 @@ cudaError_t launch_bn_relu_maxpool_fwd(const void* x, void* y, void* taps, int N
                                bn.save_mean, bn.save_invstd, ws, stream);
     if (e != cudaSuccess) return e;
     return launch_maxpool_fwd(x, y, taps, N, H, W, C, stream, bn.save_mean, bn.save_invstd, bn.gamma, bn.beta);
+}
+
+static BnEvalArgs eval_args(const void* x, const void* res, int C, const float* scale, const float* shift, int relu,
+                            const float* sc_scale, const float* sc_shift) {
+    BnEvalArgs a{};
+    a.x = static_cast<const uint4*>(x); a.res = static_cast<const uint4*>(res);
+    a.C = C; a.relu = relu;
+    a.scale = scale; a.shift = shift; a.scale2 = sc_scale; a.shift2 = sc_shift;
+    return a;
+}
+
+cudaError_t launch_bn_eval_act(const void* x, const void* res, void* y, long long M, int C, const float* scale,
+                               const float* shift, int relu, const float* sc_scale, const float* sc_shift,
+                               cudaStream_t stream) {
+    if (!bn_shape_ok(M, C)) return cudaErrorNotSupported;
+    BnEvalArgs a = eval_args(x, res, C, scale, shift, relu, sc_scale, sc_shift);
+    a.y = static_cast<uint4*>(y);
+    a.V = M * (C >> 3);
+    const int grid = bn_apply_grid(a.V, kBnApplyUnroll, kBnApplyCtas);
+    if (sc_scale != nullptr) bn_eval_kernel<true><<<grid, kBnThreads, 0, stream>>>(a);
+    else bn_eval_kernel<false><<<grid, kBnThreads, 0, stream>>>(a);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_bn_eval_act_avgpool(const void* x, const void* res, float* feat, int N, int HW, int C,
+                                       const float* scale, const float* shift, int relu, const float* sc_scale,
+                                       const float* sc_shift, cudaStream_t stream) {
+    if (N < 1 || HW < 1 || !bn_shape_ok((long long)N * HW, C)) return cudaErrorNotSupported;
+    BnEvalArgs a = eval_args(x, res, C, scale, shift, relu, sc_scale, sc_shift);
+    a.feat = feat;
+    a.HW = HW;
+    a.V = (long long)N * (C >> 3);
+    const long long blocks = (a.V + kBnPoolThreads - 1) / kBnPoolThreads;
+    if (blocks > 0x7fffffffLL) return cudaErrorNotSupported;
+    if (sc_scale != nullptr) bn_eval_avgpool_kernel<true><<<(unsigned int)blocks, kBnPoolThreads, 0, stream>>>(a);
+    else bn_eval_avgpool_kernel<false><<<(unsigned int)blocks, kBnPoolThreads, 0, stream>>>(a);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_bn_relu_maxpool_eval(const void* x, void* y, int N, int H, int W, int C, const float* scale,
+                                        const float* shift, cudaStream_t stream) {
+    if (N < 1 || H < 1 || W < 1 || !bn_shape_ok((long long)N * H * W, C)) return cudaErrorNotSupported;
+    return launch_maxpool_fwd(x, y, nullptr, N, H, W, C, stream, nullptr, nullptr, nullptr, nullptr, scale, shift);
 }
 
 }  // namespace moco

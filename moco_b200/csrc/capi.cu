@@ -617,6 +617,68 @@ int moco_bn_relu_maxpool_fwd_train(const void* x, void* y, void* taps, int N, in
     return MOCO_OK;
 }
 
+// the frozen BatchNorm entry points: scale / shift required, the shortcut's pair both or neither (and only with a
+// residual to apply it to)
+static bool bn_eval_coefs_ok(const float* scale, const float* shift, const void* residual, const float* sc_scale,
+                             const float* sc_shift) {
+    return scale && shift && (sc_scale == nullptr) == (sc_shift == nullptr) && (sc_scale == nullptr || residual);
+}
+
+int moco_bn_eval_act(const void* x, const void* residual, void* y, long long M, int C, const float* scale,
+                     const float* shift, int relu, const float* sc_scale, const float* sc_shift, void* stream_) {
+    g_err[0] = 0;
+    if (!x || !y || !bn_eval_coefs_ok(scale, shift, residual, sc_scale, sc_shift) || misaligned16(x) ||
+        misaligned16(residual) || misaligned16(y) || x == y || residual == y) {
+        set_error("moco_bn_eval_act: bad argument (null / misaligned pointer, in-place, one of sc_scale / sc_shift, "
+                  "a shortcut BN without a residual)");
+        return MOCO_ERR_INVALID;
+    }
+    cudaError_t e = launch_bn_eval_act(x, residual, y, M, C, scale, shift, relu, sc_scale, sc_shift,
+                                       static_cast<cudaStream_t>(stream_));
+    if (e == cudaErrorNotSupported) {
+        set_error("moco_bn_eval_act: needs M >= 1 and C a power of two in [64, 2048] (M=%lld C=%d)", M, C);
+        return MOCO_ERR_UNSUPPORTED;
+    }
+    if (e != cudaSuccess) return cuda_fail("batch-norm eval kernel", e);
+    return MOCO_OK;
+}
+
+int moco_bn_relu_maxpool_eval(const void* x, void* y, int N, int H, int W, int C, const float* scale,
+                              const float* shift, void* stream_) {
+    g_err[0] = 0;
+    if (!x || !y || !scale || !shift || misaligned16(x) || misaligned16(y) || x == y) {
+        set_error("moco_bn_relu_maxpool_eval: bad argument (null / misaligned pointer, in-place)");
+        return MOCO_ERR_INVALID;
+    }
+    cudaError_t e = launch_bn_relu_maxpool_eval(x, y, N, H, W, C, scale, shift, static_cast<cudaStream_t>(stream_));
+    if (e == cudaErrorNotSupported) {
+        set_error("moco_bn_relu_maxpool_eval: needs N, H, W >= 1 and C a power of two in [64, 2048] (C=%d)", C);
+        return MOCO_ERR_UNSUPPORTED;
+    }
+    if (e != cudaSuccess) return cuda_fail("batch-norm eval + max-pool kernel", e);
+    return MOCO_OK;
+}
+
+int moco_bn_eval_act_avgpool(const void* x, const void* residual, float* feat, int N, int HW, int C, const float* scale,
+                             const float* shift, int relu, const float* sc_scale, const float* sc_shift, void* stream_) {
+    g_err[0] = 0;
+    if (!x || !feat || !bn_eval_coefs_ok(scale, shift, residual, sc_scale, sc_shift) || misaligned16(x) ||
+        misaligned16(residual) || misaligned16(feat)) {
+        set_error("moco_bn_eval_act_avgpool: bad argument (null / misaligned pointer, one of sc_scale / sc_shift, "
+                  "a shortcut BN without a residual)");
+        return MOCO_ERR_INVALID;
+    }
+    cudaError_t e = launch_bn_eval_act_avgpool(x, residual, feat, N, HW, C, scale, shift, relu, sc_scale, sc_shift,
+                                               static_cast<cudaStream_t>(stream_));
+    if (e == cudaErrorNotSupported) {
+        set_error("moco_bn_eval_act_avgpool: needs N, HW >= 1 and C a power of two in [64, 2048] (N=%d HW=%d C=%d)", N,
+                  HW, C);
+        return MOCO_ERR_UNSUPPORTED;
+    }
+    if (e != cudaSuccess) return cuda_fail("batch-norm eval + average-pool kernel", e);
+    return MOCO_OK;
+}
+
 int moco_crop_to_nhwc_bf16(const void* src, int src_dtype, long long src_image_stride, void* dst, int N, int C, int HW,
                            void* stream_) {
     g_err[0] = 0;

@@ -93,10 +93,13 @@ cudaError_t launch_enqueue(__nv_bfloat16* queue_bf16, float* queue_f32, const vo
                            int n_all, int C, int64_t K, int64_t index, int64_t shard_row0, int64_t shard_rows,
                            cudaStream_t stream);
 cudaError_t launch_f32_to_bf16(const float* src, __nv_bfloat16* dst, size_t n, cudaStream_t stream);
-// bn_*: nullable; the stem's BatchNorm + ReLU applied to each tap (moco_bn_relu_maxpool_fwd_train)
+// bn_*: nullable; the stem's BatchNorm + ReLU applied to each tap (moco_bn_relu_maxpool_fwd_train).
+// eval_scale / eval_shift: nullable; the same with a frozen BatchNorm's folded coefficients (moco_bn_relu_maxpool_eval),
+// idx may then be NULL (no tap bytes are written).
 cudaError_t launch_maxpool_fwd(const void* x, void* y, void* idx, int N, int H, int W, int C, cudaStream_t stream,
                                const float* bn_mean = nullptr, const float* bn_invstd = nullptr,
-                               const float* bn_gamma = nullptr, const float* bn_beta = nullptr);
+                               const float* bn_gamma = nullptr, const float* bn_beta = nullptr,
+                               const float* eval_scale = nullptr, const float* eval_shift = nullptr);
 cudaError_t launch_maxpool_bwd(const void* dy, const void* idx, void* dx, int N, int H, int W, int C, cudaStream_t stream);
 cudaError_t launch_crop_to_s2d(const void* src, int src_dtype, long long img_stride, __nv_bfloat16* dst, int N, int H, int W,
                                cudaStream_t stream, const int64_t* src_rows);
@@ -115,6 +118,14 @@ cudaError_t launch_bn_add_relu_bwd(const void* dy, const void* x, const void* re
                                    cudaStream_t stream);
 cudaError_t launch_bn_relu_maxpool_fwd(const void* x, void* y, void* taps, int N, int H, int W, int C, const BnLayer& bn,
                                        void* ws, cudaStream_t stream);
+cudaError_t launch_bn_eval_act(const void* x, const void* res, void* y, long long M, int C, const float* scale,
+                               const float* shift, int relu, const float* sc_scale, const float* sc_shift,
+                               cudaStream_t stream);
+cudaError_t launch_bn_eval_act_avgpool(const void* x, const void* res, float* feat, int N, int HW, int C,
+                                       const float* scale, const float* shift, int relu, const float* sc_scale,
+                                       const float* sc_shift, cudaStream_t stream);
+cudaError_t launch_bn_relu_maxpool_eval(const void* x, void* y, int N, int H, int W, int C, const float* scale,
+                                        const float* shift, cudaStream_t stream);
 int ema_chunk_elems();
 cudaError_t launch_ema(const void* segs, const int* chunk_prefix, int n_segs, int n_chunks, float m,
                        float one_minus_m, cudaStream_t stream);

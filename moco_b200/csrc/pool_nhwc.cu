@@ -30,6 +30,10 @@ struct PoolArgs {
     const float* invstd;
     const float* gamma;
     const float* beta;
+    // forward, nullable: a frozen BatchNorm's folded scale / shift applied to every tap by the header's eval contract
+    // (moco_bn_relu_maxpool_eval); idx is then NULL
+    const float* scale;
+    const float* shift;
 };
 
 __device__ __forceinline__ void unpack8p(const uint4& u, float* f) {
@@ -52,15 +56,18 @@ maxpool3x3s2_fwd_kernel(const PoolArgs a) {
     p /= a.OW;
     const int oh = (int)(p % a.OH);
     const int n = (int)(p / a.OH);
-    const bool bn = a.gamma != nullptr;
+    const bool bn = a.gamma != nullptr, ev = a.scale != nullptr;
     float ca[8], cb[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) {
         ca[k] = cb[k] = 0.f;
+        const int c = cv * 8 + k;
         if (bn) {
-            const int c = cv * 8 + k;
             ca[k] = __ldg(a.gamma + c) * __ldg(a.invstd + c);
             cb[k] = fmaf(-__ldg(a.mean + c), ca[k], __ldg(a.beta + c));
+        } else if (ev) {
+            ca[k] = __ldg(a.scale + c);
+            cb[k] = __ldg(a.shift + c);
         }
     }
     float m[8];
@@ -83,6 +90,12 @@ maxpool3x3s2_fwd_kernel(const PoolArgs a) {
 #pragma unroll
                 for (int k = 0; k < 8; ++k)       // bn_apply_kernel's relu(x * ca + cb + 0), rounded to bf16
                     f[k] = __bfloat162float(__float2bfloat16_rn(fmaxf(__fadd_rn(fmaf(f[k], ca[k], cb[k]), 0.f), 0.f)));
+            } else if (ev) {
+#pragma unroll
+                for (int k = 0; k < 8; ++k) {     // bn_eval_kernel's relu(x * s + t): no FMA, rounded to bf16
+                    const float z = __fadd_rn(__fmul_rn(f[k], ca[k]), cb[k]);
+                    f[k] = __bfloat162float(__float2bfloat16_rn(z > 0.f ? z : 0.f));
+                }
             }
             const unsigned int t = (unsigned int)(kh * 3 + kw);
 #pragma unroll
@@ -98,6 +111,7 @@ maxpool3x3s2_fwd_kernel(const PoolArgs a) {
 #pragma unroll
     for (int k = 0; k < 4; ++k) h[k] = __floats2bfloat162_rn(m[2 * k], m[2 * k + 1]);
     a.y[o] = out;
+    if (a.idx == nullptr) return;                // eval: no backward follows
     uint2 ix;
     ix.x = tap[0] | (tap[1] << 8) | (tap[2] << 16) | (tap[3] << 24);
     ix.y = tap[4] | (tap[5] << 8) | (tap[6] << 16) | (tap[7] << 24);
@@ -155,11 +169,13 @@ static bool pool_shape(int N, int H, int W, int C, PoolArgs* a) {
 }
 
 cudaError_t launch_maxpool_fwd(const void* x, void* y, void* idx, int N, int H, int W, int C, cudaStream_t stream,
-                               const float* bn_mean, const float* bn_invstd, const float* bn_gamma, const float* bn_beta) {
+                               const float* bn_mean, const float* bn_invstd, const float* bn_gamma, const float* bn_beta,
+                               const float* eval_scale, const float* eval_shift) {
     PoolArgs a{};
     if (!pool_shape(N, H, W, C, &a)) return cudaErrorNotSupported;
     a.x = static_cast<const uint4*>(x); a.y = static_cast<uint4*>(y); a.idx = static_cast<uint2*>(idx);
     a.mean = bn_mean; a.invstd = bn_invstd; a.gamma = bn_gamma; a.beta = bn_beta;
+    a.scale = eval_scale; a.shift = eval_shift;
     a.total = (long long)N * a.OH * a.OW * a.lanes;
     const long long blocks = (a.total + kPoolThreads - 1) / kPoolThreads;
     if (blocks > 0x7fffffffLL) return cudaErrorNotSupported;
