@@ -48,9 +48,9 @@ enum {
     MOCO_NCE_SINGLE_CTA = 4,   /* require the tensor-core path (error instead of the generic fallback) */
     MOCO_NCE_TWO_PASS = 512,   /* statistics pass, then dq pass normalised with the final lse (always exact) */
     MOCO_NCE_ONE_PASS = 1024   /* loss AND dq from one sweep over the queue (4NCK FLOP, NK exps instead of   */
-                               /* 6NCK, 2NK) plus ONE tail kernel: each (CTA, row) stabilises with the row   */
-                               /* maximum of the CTA's first tile.  A row whose partial sum leaves the safe  */
-                               /* range (a later logit > ~100 binades above that maximum: un-normalised      */
+                               /* 6NCK, 2NK) plus ONE tail kernel: every row stabilises with the constant    */
+                               /* log2e * inv_T.  A row whose partial sum leaves the safe range (a logit     */
+                               /* > ~100 binades above it, or all logits far below it: un-normalised         */
                                /* inputs) is detected by the tail kernel and recomputed exactly on CUDA      */
                                /* cores, so the result always equals the reference's.  AUTO picks it when dq */
                                /* is requested, logits are not, and inv_T <= MOCO_ONE_PASS_MAX_INV_T (with   */
@@ -182,7 +182,14 @@ int moco_queue_enqueue(void* queue_bf16, float* queue_f32_or_null,
  * (it also leaves the unnormalised P~.Queue partials in the workspace) and the
  * dq call just rescales and sums them with the merged lse -- the caller must not
  * use the workspace for anything else in between (moco_nce_shard_merge is fine).
- * Same numerical contract as MOCO_NCE_ONE_PASS of moco_nce_fwd.
+ * Same numerical contract as MOCO_NCE_ONE_PASS of moco_nce_fwd: exact for any q.  A row one of whose slice
+ * sums is above 2^100 or NaN, or whose shard sum is below 2^-80 (relative to the sweep's constant stabiliser
+ * log2e * inv_T), is evaluated exactly on CUDA cores: the statistics call writes that row's exact
+ * (log2 sum_{j in shard} 2^x_ij, 1) into ms_out and records the decision in the workspace, and the dq call
+ * computes that row's o_partial exactly against the shard with the merged lse.  Same launches either way.
+ *
+ * moco_nce_shard_merge: world in [1, 160].  moco_nce_shard_dq_finish_peers: world in [1, 16], 0 <= rank < world,
+ * every peer pointer non-NULL and 16-byte aligned, C a multiple of 4.
  *
  * The loss is permutation-invariant over negatives, so it equals the replicated
  * reference's; ring slot g of moco/NCE/Contrast.py:32 maps to (rank g / (K/W),

@@ -345,16 +345,19 @@ int moco_nce_shard_stats(const void* q_all, const void* k_all, int qk_dtype, con
     p.cta_group = (flags & MOCO_NCE_CTA_PAIR) ? 2 : 1;
     p.num_sms = d.sms;
     p.slices = 0; p.n_pad = 0;
+    ShardExact exact = {nullptr, p.q_bf16, p.queue, Ks, inv_T};
     if (flags & MOCO_NCE_ONE_PASS) {
         // one sweep over the shard: (stabiliser, sum) partials for the cross-rank merge AND the unnormalised
-        // P~.Queue partials, which stay in the workspace until moco_nce_shard_dq(..., MOCO_NCE_ONE_PASS) rescales them
+        // P~.Queue partials, which stay in the workspace until moco_nce_shard_dq(..., MOCO_NCE_ONE_PASS) rescales them;
+        // rows outside the sweep's safe range are evaluated exactly by the combine kernel (and by the dq call)
         e = launch_sweep(q_all, qk_dtype, 0, p.q_bf16, p.queue, N, C, Ks, inv_T, nullptr, d.sms, &p.slices, &p.n_pad, ws, stream);
         if (e != cudaSuccess) return cuda_fail("one-pass kernel", e);
+        exact.row_exact = ws.row_exact;
     } else {
         e = launch_nce_tc(p, ws, stream);
         if (e != cudaSuccess) return cuda_fail("statistics kernel", e);
     }
-    e = launch_combine_partial(N, p.slices, p.n_pad, static_cast<float2*>(ms_out), ws, stream);
+    e = launch_combine_partial(N, C, p.slices, p.n_pad, static_cast<float2*>(ms_out), ws, exact, stream);
     if (e != cudaSuccess) return cuda_fail("combine kernel", e);
     return MOCO_OK;
 }
@@ -363,7 +366,7 @@ int moco_nce_shard_merge(const void* ms_all, int world, int N, int C, float inv_
                          float* prob_rows, float* loss_prob, void* workspace, size_t workspace_bytes, void* stream_) {
     g_err[0] = 0;
     if (!ms_all || !lse || !loss_rows || !prob_rows || !loss_prob || !workspace || world < 1 || world > kMaxCtas || N <= 0) {
-        set_error("moco_nce_shard_merge: bad argument");
+        set_error("moco_nce_shard_merge: bad argument (null pointer, N=%d, or world=%d outside [1, %d])", N, world, kMaxCtas);
         return MOCO_ERR_INVALID;
     }
     NceWorkspace ws = carve_workspace(workspace, N, C);
@@ -389,11 +392,13 @@ int moco_nce_shard_dq(const void* q_all, int q_dtype, const void* shard_bf16, co
     cudaError_t e;
     if (flags & MOCO_NCE_ONE_PASS) {
         // the sweep already happened in moco_nce_shard_stats(..., MOCO_NCE_ONE_PASS) on this workspace: only the
-        // slice count is needed, then O = sum_s 2^(m_s - lse) O~_s
+        // slice count is needed, then O = sum_s 2^(m_s - lse) O~_s (exactly, for the rows that call flagged)
         e = launch_sweep(q_all, q_dtype, 0, qb, static_cast<const __nv_bfloat16*>(shard_bf16), N, C, Ks, inv_T, nullptr, d.sms,
                          &slices, &n_pad, ws, stream, /*plan_only=*/true);
         if (e != cudaSuccess) return cuda_fail("one-pass plan", e);
-        e = launch_dq_reduce(N, C, slices, n_pad, inv_T, nullptr, 0, nullptr, o_partial, ws.part_o, stream, ws.part_ms, lse_all);
+        const ShardExact exact = {ws.row_exact, qb, static_cast<const __nv_bfloat16*>(shard_bf16), Ks, inv_T};
+        e = launch_dq_reduce(N, C, slices, n_pad, inv_T, nullptr, 0, nullptr, o_partial, ws.part_o, stream, ws.part_ms,
+                             lse_all, exact);
         if (e != cudaSuccess) return cuda_fail("dq reduce kernel", e);
         return MOCO_OK;
     }
@@ -423,7 +428,8 @@ int moco_nce_shard_dq_finish_peers(const void* const* o_peers_host, int world, i
     g_err[0] = 0;
     if (!o_peers_host || !k_own || !prob_rows_own || !dq || N <= 0 || C <= 0 || (C & 3) || world < 1 || world > 16 ||
         rank < 0 || rank >= world) {
-        set_error("moco_nce_shard_dq_finish_peers: bad argument");
+        set_error("moco_nce_shard_dq_finish_peers: bad argument (null pointer, N=%d, C=%d not a multiple of 4, or "
+                  "world=%d / rank=%d outside 1 <= world <= 16, 0 <= rank < world)", N, C, world, rank);
         return MOCO_ERR_INVALID;
     }
     for (int r = 0; r < world; ++r)

@@ -23,7 +23,19 @@ struct NceWorkspace {
     __nv_bfloat16* q_bf16;    // [N, C] bf16 copy of q (when q arrives as fp32)
     float2* part_ms;          // [slices, N_pad] per-slice (running max, sum) in the log2 domain
     float* part_o;            // [slices, N_pad, C] per-slice unnormalised sum_j 2^(x_ij - m) queue_j
+    int* row_exact;           // [N]   sharded one-sweep mode: 1 where the statistics call evaluated the row exactly,
+                              //       so the dq call must too (ShardExact below)
     size_t bytes;
+};
+
+// Exact CUDA-core evaluation of the rows the sharded one-sweep kernel cannot represent (moco_nce_shard_stats /
+// moco_nce_shard_dq with MOCO_NCE_ONE_PASS).  row_exact == nullptr: no such evaluation (two-pass mode).
+struct ShardExact {
+    int* row_exact;                  // [N] per-row decision, written by the statistics call, read by the dq call
+    const __nv_bfloat16* q;          // [N, C] bf16(q)
+    const __nv_bfloat16* shard;      // [Ks, C]
+    int Ks;
+    float inv_T;
 };
 
 // Programmatic dependent launch for the head's kernel chain (prep -> one-pass | stats -> combine [-> dq] -> dq_reduce
@@ -64,6 +76,7 @@ inline NceWorkspace carve_workspace(void* base, int N, int C) {
     w.q_bf16 = reinterpret_cast<__nv_bfloat16*>(p + off);             off += align_up((size_t)N * C * 2, 256);
     w.part_ms = reinterpret_cast<float2*>(p + off);                   off += align_up((size_t)kMaxCtas * kRowsPerCta * 8, 256);
     w.part_o = reinterpret_cast<float*>(p + off);                     off += align_up((size_t)kMaxCtas * kRowsPerCta * C * 4, 256);
+    w.row_exact = reinterpret_cast<int*>(p + off);                    off += align_up((size_t)N * 4, 256);
     w.bytes = off;
     return w;
 }
@@ -80,11 +93,12 @@ cudaError_t launch_combine(int N, int C, int slices, int n_pad, float inv_T, flo
                            const NceWorkspace& ws, cudaStream_t stream);
 cudaError_t launch_dq_reduce(int N, int C, int slices, int n_pad, float inv_T, const void* k, int k_dtype,
                              const float* prob_rows, float* dq, const float* part_o, cudaStream_t stream,
-                             const float2* part_ms = nullptr, const float* lse = nullptr);
+                             const float2* part_ms = nullptr, const float* lse = nullptr,
+                             const ShardExact& exact = ShardExact{nullptr, nullptr, nullptr, 0, 0.f});
 cudaError_t launch_dq_finish_peers(const void* const* peers_host, int world, int rank, int N, int C, float inv_T,
                                    const void* k, int k_dtype, const float* prob_rows, float* dq, cudaStream_t stream);
-cudaError_t launch_combine_partial(int N, int slices, int n_pad, float2* ms_out, const NceWorkspace& ws,
-                                   cudaStream_t stream);
+cudaError_t launch_combine_partial(int N, int C, int slices, int n_pad, float2* ms_out, const NceWorkspace& ws,
+                                   const ShardExact& exact, cudaStream_t stream);
 cudaError_t launch_combine_merge(int N, int world, float inv_T, const float2* ms_all, float* lse, float* loss_rows,
                                  float* prob_rows, float* loss_prob, const NceWorkspace& ws, cudaStream_t stream);
 cudaError_t launch_bwd_dense(const float* g, const void* k, int k_dtype, const __nv_bfloat16* queue,

@@ -61,6 +61,11 @@ __device__ inline bool finish_mean(unsigned int* counter, int N, const float* lo
 constexpr int kSimtThreads = 256;
 constexpr int kSimtMaxC = 1024;
 
+// Safe range of the one-sweep kernel's per-row sums (fixed stabiliser, see nce_sweep_sm90.cu): a row with a slice sum
+// above kOnePassUnsafeSum (or NaN), or a merged sum below kOnePassUnderflow, is evaluated exactly on CUDA cores instead.
+constexpr float kOnePassUnsafeSum = 1.2676506e30f;    // 2^100
+constexpr float kOnePassUnderflow = 8.2718061e-25f;   // 2^-80
+
 __device__ __forceinline__ float dot_row(const float* __restrict__ qs, const __nv_bfloat16* __restrict__ row, int C) {
     float acc = 0.f;
     if ((C & 7) == 0) {

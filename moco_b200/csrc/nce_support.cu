@@ -52,28 +52,11 @@ __global__ void combine_kernel(int N, int C, int K, int slices, int n_pad, float
                                float* __restrict__ logits,
                                float* __restrict__ lse, float* __restrict__ loss_rows,
                                float* __restrict__ prob_rows, float* __restrict__ loss_prob,
-                               unsigned int* __restrict__ counters, float2* __restrict__ ms_out) {
+                               unsigned int* __restrict__ counters) {
     pdl_launch_dependents();
     pdl_wait();
     const int i = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);     // one warp per q row
     const float scale2 = inv_T * kLog2e;
-    if (ms_out != nullptr) {
-        // partial mode (sharded queue): merge this rank's slices only -> one (max, sum) per row, no positive
-        if (i < N) {
-            int lane = threadIdx.x & 31;
-            float m = -INFINITY;
-            for (int s = lane; s < slices; s += 32) m = fmaxf(m, part_ms[(size_t)s * n_pad + i].x);
-            m = warp_max(m);
-            float l = 0.f;
-            for (int s = lane; s < slices; s += 32) {
-                float2 ms = part_ms[(size_t)s * n_pad + i];
-                if (ms.x != -INFINITY) l += ms.y * ex2(ms.x - m);
-            }
-            l = warp_sum(l);
-            if (lane == 0) ms_out[i] = make_float2(m, l);
-        }
-        return;
-    }
     if (i < N) {
         const float x0 = lpos[i] * scale2;         // positive logit, log2 domain
         int lane = threadIdx.x & 31;
@@ -107,15 +90,60 @@ cudaError_t launch_combine(int N, int C, int slices, int n_pad, float inv_T, flo
     const int rows_per_block = 8;
     return launch_pdl(combine_kernel, dim3((N + rows_per_block - 1) / rows_per_block), dim3(rows_per_block * 32), 0,
                       stream, N, C, K, slices, n_pad, inv_T, ws.lpos, ws.part_ms, logits, lse, loss_rows, prob_rows,
-                      loss_prob, ws.counters, nullptr);
+                      loss_prob, ws.counters);
 }
 
-// sharded queue, step 1: this rank's slices -> ms_out[N]
-cudaError_t launch_combine_partial(int N, int slices, int n_pad, float2* ms_out, const NceWorkspace& ws,
-                                   cudaStream_t stream) {
-    const int rows_per_block = 8;
-    combine_kernel<<<(N + rows_per_block - 1) / rows_per_block, rows_per_block * 32, 0, stream>>>(
-        N, 0, 0, slices, n_pad, 1.f, nullptr, ws.part_ms, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, ms_out);
+// Sharded queue, step 1: merge this rank's slices only -> one (max, sum) per row, no positive.  One warp per row.
+// With ex.row_exact (one-sweep mode) a row whose sums left the one-sweep kernel's safe range is flagged there and
+// evaluated exactly against the shard by the whole block: ms_out = (log2 of the shard's sum, 1).
+constexpr int kPartialRows = 8;
+static_assert(kPartialRows * 32 == kSimtThreads, "the exact evaluation takes the whole block");
+
+__global__ void __launch_bounds__(kPartialRows * 32)
+combine_partial_kernel(int N, int C, int slices, int n_pad, const float2* __restrict__ part_ms,
+                       float2* __restrict__ ms_out, const ShardExact ex) {
+    __shared__ SimtRowSmem sm;
+    __shared__ int s_exact[kPartialRows];
+    const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int i = blockIdx.x * kPartialRows + w;
+    bool exact = false;
+    if (i < N) {
+        float m = -INFINITY, lmax = 0.f;
+        for (int s = lane; s < slices; s += 32) m = fmaxf(m, part_ms[(size_t)s * n_pad + i].x);
+        m = warp_max(m);
+        float l = 0.f;
+        for (int s = lane; s < slices; s += 32) {
+            float2 ms = part_ms[(size_t)s * n_pad + i];
+            if (ms.x != -INFINITY) l += ms.y * ex2(ms.x - m);
+            lmax = fmaxf(lmax, (ms.y == ms.y) ? ms.y : INFINITY);                // NaN counts as unsafe
+        }
+        l = warp_sum(l);
+        if (ex.row_exact != nullptr) {
+            lmax = warp_max(lmax);
+            exact = lmax > kOnePassUnsafeSum || !(l >= kOnePassUnderflow);
+            if (lane == 0) ex.row_exact[i] = exact ? 1 : 0;
+        }
+        if (lane == 0 && !exact) ms_out[i] = make_float2(m, l);
+    }
+    if (ex.row_exact == nullptr) return;
+    if (lane == 0) s_exact[w] = exact ? 1 : 0;
+    __syncthreads();
+    for (int r = 0; r < kPartialRows; ++r) {                  // rare: the block's branch is uniform
+        if (!s_exact[r]) continue;
+        const int row = blockIdx.x * kPartialRows + r;
+        for (int c = threadIdx.x; c < C; c += blockDim.x) sm.qs[c] = __bfloat162float(ex.q[(size_t)row * C + c]);
+        __syncthreads();
+        const float lse2 = simt_row_stats(sm, -INFINITY, ex.shard, C, ex.Ks, ex.inv_T, nullptr);
+        if (threadIdx.x == 0) ms_out[row] = make_float2(lse2, 1.f);
+        __syncthreads();                                      // sm is reused by the next flagged row
+    }
+}
+
+cudaError_t launch_combine_partial(int N, int C, int slices, int n_pad, float2* ms_out, const NceWorkspace& ws,
+                                   const ShardExact& exact, cudaStream_t stream) {
+    if (exact.row_exact != nullptr && C > kSimtMaxC) return cudaErrorNotSupported;
+    combine_partial_kernel<<<(N + kPartialRows - 1) / kPartialRows, kPartialRows * 32, 0, stream>>>(
+        N, C, slices, n_pad, ws.part_ms, ms_out, exact);
     return cudaGetLastError();
 }
 
@@ -124,23 +152,45 @@ cudaError_t launch_combine_merge(int N, int world, float inv_T, const float2* ms
                                  float* prob_rows, float* loss_prob, const NceWorkspace& ws, cudaStream_t stream) {
     const int rows_per_block = 8;
     combine_kernel<<<(N + rows_per_block - 1) / rows_per_block, rows_per_block * 32, 0, stream>>>(
-        N, 0, 0, world, N, inv_T, ws.lpos, ms_all, nullptr, lse, loss_rows, prob_rows, loss_prob, ws.counters, nullptr);
+        N, 0, 0, world, N, inv_T, ws.lpos, ms_all, nullptr, lse, loss_rows, prob_rows, loss_prob, ws.counters);
     return cudaGetLastError();
+}
+
+// o_partial_i = sum_{j in shard} p_ij shard_j of one row, exactly (out of line: the common path keeps its registers)
+__device__ __noinline__ void shard_exact_row_o(SimtRowSmem& sm, const __nv_bfloat16* __restrict__ q_row,
+                                               const __nv_bfloat16* __restrict__ shard, int Ks, int C, float inv_T,
+                                               float lse2, float* __restrict__ o_row) {
+    for (int c = threadIdx.x; c < C; c += blockDim.x) sm.qs[c] = __bfloat162float(q_row[c]);
+    __syncthreads();
+    float acc[kSimtMaxC / kSimtThreads];
+    simt_row_grad(sm, lse2, shard, C, Ks, inv_T, acc);
+#pragma unroll
+    for (int u = 0; u < kSimtMaxC / kSimtThreads; ++u) {
+        const int c = threadIdx.x + u * kSimtThreads;
+        if (c < C) o_row[c] = acc[u];
+    }
 }
 
 // dq_i = inv_T / N * ( sum_slices w_s O_s[i] + (prob_i - 1) k_i )   -- fixed summation order.
 // w_s = 1 when the dq kernel normalised with the final lse (two-pass); in one-pass mode slice s used its own
-// stabiliser m_s (part_ms[s][i].x, log2 domain) and w_s = 2^(m_s - lse_i) finishes the normalisation here.
-__global__ void dq_reduce_kernel(int N, int C, int slices, int n_pad, float inv_T, const void* __restrict__ k,
-                                 int k_dtype, const float* __restrict__ part_o,
-                                 const float* __restrict__ prob_rows, float* __restrict__ dq,
-                                 const float2* __restrict__ part_ms, const float* __restrict__ lse) {
+// stabiliser m_s (part_ms[s][i].x, log2 domain) and w_s = 2^(m_s - lse_i) finishes the normalisation here, except
+// for the rows the sharded statistics call evaluated exactly (ex.row_exact): those are evaluated exactly here too.
+__global__ void __launch_bounds__(kSimtThreads, 8)      // full occupancy: the exact branch is out of line
+dq_reduce_kernel(int N, int C, int slices, int n_pad, float inv_T, const void* __restrict__ k,
+                 int k_dtype, const float* __restrict__ part_o,
+                 const float* __restrict__ prob_rows, float* __restrict__ dq,
+                 const float2* __restrict__ part_ms, const float* __restrict__ lse, const ShardExact ex) {
     // 256 threads = (C/4 float4 lanes) x groups; group g sums slices g, g+groups, ...; groups are then
     // added in index order (deterministic).
-    __shared__ float4 s_part[256];
+    __shared__ union { float4 part[256]; SimtRowSmem row; } sh;
+    float4* s_part = sh.part;
     pdl_launch_dependents();
     pdl_wait();
     const int i = blockIdx.x;
+    if (ex.row_exact != nullptr && ex.row_exact[i]) {      // raw mode (o_partial), block-uniform branch
+        shard_exact_row_o(sh.row, ex.q + (size_t)i * C, ex.shard, ex.Ks, C, ex.inv_T, lse[i] * kLog2e, dq + (size_t)i * C);
+        return;
+    }
     const int lanes = C >> 2;
     const int groups = 256 / lanes;
     const int lane = threadIdx.x % lanes, grp = threadIdx.x / lanes;
@@ -183,10 +233,10 @@ __global__ void dq_reduce_kernel(int N, int C, int slices, int n_pad, float inv_
 
 cudaError_t launch_dq_reduce(int N, int C, int slices, int n_pad, float inv_T, const void* k, int k_dtype,
                              const float* prob_rows, float* dq, const float* part_o, cudaStream_t stream,
-                             const float2* part_ms, const float* lse) {
+                             const float2* part_ms, const float* lse, const ShardExact& exact) {
     if ((C & 3) != 0 || C > 1024) return cudaErrorNotSupported;
-    return launch_pdl(dq_reduce_kernel, dim3(N), dim3(256), 0, stream, N, C, slices, n_pad, inv_T, k, k_dtype, part_o,
-                      prob_rows, dq, part_ms, lse);
+    return launch_pdl(dq_reduce_kernel, dim3(N), dim3(kSimtThreads), 0, stream, N, C, slices, n_pad, inv_T, k, k_dtype,
+                      part_o, prob_rows, dq, part_ms, lse, exact);
 }
 
 // Sharded queue, last step: dq_i = inv_T / N * ( sum_r O_r[row0 + i] + (prob_i - 1) k_i ), the W partial-gradient

@@ -19,12 +19,12 @@
 // This kernel WRITES the queue, so it never triggers its dependents early: the next kernel that reads the queue
 // starts after it has completed.
 //
-// Exactness: the head kernels work with a per-row exponent offset m (C <= 128: the bound log2e/T |q_i|; C > 128: the
-// row maximum of the CTA's first tile).  If a slice's partial sum left the safe range (> 2^100: logits far above m) or
-// the merged sum is so small that flushed terms could matter (< 2^-80 relative to the largest exponent: logits far
-// below the bound, e.g. un-normalised q), the row falls back to the exact CUDA-core evaluation of that row against
-// the whole queue (nce_rows.cuh): the one-sweep path is never silently wrong and never returns inf/NaN where the
-// reference would not.  With L2-normalised features neither happens.
+// Exactness: the sweep kernel works with the constant exponent offset m = log2e/T for every row and every C (the
+// largest logit of a unit-norm query against a unit-norm queue row).  If a slice's partial sum left the safe range
+// (> 2^100: logits far above m) or the merged sum is so small that flushed terms could matter (< 2^-80 relative to
+// the largest exponent: logits far below the bound, e.g. un-normalised q), the row falls back to the exact CUDA-core
+// evaluation of that row against the whole queue (nce_rows.cuh): the one-sweep path is never silently wrong and never
+// returns inf/NaN where the reference would not.  With L2-normalised features neither happens.
 #include "../../include/moco_b200.h"
 #include "common.cuh"
 #include "nce_rows.cuh"
@@ -35,8 +35,6 @@ namespace moco {
 constexpr int kTailThreads = kSimtThreads;         // 256
 constexpr int kMaxTailDevices = 64;
 constexpr int kTailMaxSlices = kMaxCtas;           // 160
-constexpr float kTailUnsafeSum = 1.2676506e30f;    // 2^100
-constexpr float kTailUnderflow = 8.2718061e-25f;   // 2^-80
 
 struct TailArgs {
     int N, C, K, slices, n_pad;
@@ -147,7 +145,7 @@ nce_tail_kernel(const TailArgs a) {
             l += ex2(x0 - m);
             if (tid == 0) {
                 s_val[0] = m + log2f(l);
-                s_val[2] = (lmax > kTailUnsafeSum || !(l >= kTailUnderflow)) ? 1.f : 0.f;
+                s_val[2] = (lmax > kOnePassUnsafeSum || !(l >= kOnePassUnderflow)) ? 1.f : 0.f;
             }
         }
         __syncthreads();
