@@ -90,7 +90,11 @@ int moco_device_info(int* sm_count, int* cc_major, int* cc_minor);
  * `logits` ([N, K+1] fp32, row stride K+1) may be NULL: then no logit ever
  * reaches HBM.  `dq` ([N, C] fp32) may be NULL.  lse / loss_rows / prob_rows:
  * [N] fp32; loss_prob: [2] fp32.  All reductions are deterministic (fixed
- * order, no float atomics).
+ * order, no float atomics).  q and queue_bf16 must be 16-byte aligned
+ * (MOCO_ERR_INVALID otherwise, before any device access).
+ * Every logit is fp32(fp32(dot) * inv_T), with dot the fp32-accumulated product:
+ * when every partial sum of a dot is exact in fp32 (e.g. operands with few
+ * power-of-two entries) the logits are bit-identical on every path.
  * ---------------------------------------------------------------------- */
 size_t moco_nce_workspace_bytes(int N, int C, int K);
 
@@ -121,9 +125,11 @@ int moco_nce_fwd(const void* q, const void* k, int qk_dtype,
  * index_dev != NULL -- read from that device int64 and advanced there
  * ((index + n_all) mod K, Contrast.py:34) by kernel 2, so a CUDA graph capturing
  * this call replays correctly step after step.  queue_f32 may be NULL.
+ * q, queue_bf16, queue_f32 and k_all must be 16-byte aligned (MOCO_ERR_INVALID
+ * otherwise, before any device access).
  * Shapes outside the one-sweep envelope fall back to the moco_nce_fwd kernels
- * followed by the enqueue kernel (then normalize and index_dev must be 0/NULL:
- * MOCO_ERR_UNSUPPORTED otherwise).
+ * followed by the enqueue kernel, which then reads and advances index_dev
+ * itself; normalize must be 0 there (MOCO_ERR_UNSUPPORTED otherwise).
  * ---------------------------------------------------------------------- */
 int moco_nce_step(const void* q, const void* k, int qk_dtype, int normalize,
                   void* queue_bf16, float* queue_f32_or_null, int N, int C, int K, float inv_T,
@@ -155,7 +161,9 @@ int moco_nce_bwd_dense(const float* grad_logits, const void* k, int k_dtype,
  * `index` is the write pointer BEFORE the call; the caller advances it
  * ((index + n_all) mod K, Contrast.py:34).  Writes the bf16 working queue and,
  * when non-NULL, the fp32 master copy (the checkpointed `memory` buffer,
- * Contrast.py:18).  Requires n_all <= K (SURVEY S10).
+ * Contrast.py:18).  Requires n_all <= K (SURVEY S10).  queue_bf16, queue_f32 and
+ * k_all must be 16-byte aligned (MOCO_ERR_INVALID otherwise); the same holds for
+ * shard_bf16, shard_f32 and k_all of moco_queue_enqueue_shard.
  * ---------------------------------------------------------------------- */
 int moco_queue_enqueue(void* queue_bf16, float* queue_f32_or_null,
                        const void* k_all, int k_dtype, int n_all, int C, int64_t K,

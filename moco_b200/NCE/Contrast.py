@@ -39,6 +39,12 @@ class _Scratch:
         self.ws_ptr = self.ws.data_ptr() + off
 
 
+def _aligned16(t):
+    """The kernels read q and k_all with 16-byte vector loads (include/moco_b200.h): a contiguous view that starts at
+    an odd storage offset is copied."""
+    return t if t.data_ptr() % 16 == 0 else t.clone()
+
+
 def _nce_forward(mod: "MemoryMoCo", q, k, want_logits: bool, want_dq: bool, flags: int, k_all=None,
                  normalize: bool = False):
     """One head evaluation.  With ``k_all`` the FIFO enqueue (Contrast.py:29-34) is part of the same C call
@@ -52,7 +58,7 @@ def _nce_forward(mod: "MemoryMoCo", q, k, want_logits: bool, want_dq: bool, flag
         raise RuntimeError(f"MemoryMoCo: q on {q.device}, k on {k.device}, queue on {mod.memory.device}")
     if q.dtype != k.dtype:
         k = k.to(q.dtype)
-    q = q.contiguous()
+    q = _aligned16(q.contiguous())
     k = k.contiguous()
     N, C = q.shape
     K = mod.queue_size
@@ -255,7 +261,7 @@ class MemoryMoCo(nn.Module):
     # -- enqueue (Contrast.py:29-34) ----------------------------------------
     def _check_keys(self, k_all):
         _lib.require_cuda(k_all)
-        k_all = k_all.detach().contiguous()
+        k_all = _aligned16(k_all.detach().contiguous())
         if k_all.dim() != 2 or k_all.shape[1] != self.memory.shape[1]:
             raise ValueError(f"MemoryMoCo: k_all {tuple(k_all.shape)} does not match the queue "
                              f"{tuple(self.memory.shape)}")

@@ -21,6 +21,7 @@ import torch.distributed as dist
 from torch import nn
 
 from .. import _lib
+from .Contrast import _aligned16
 
 
 def _world():
@@ -309,7 +310,7 @@ class ShardedMemoryMoCo(nn.Module):
     def enqueue(self, k_all):
         lib = _lib.load()
         _lib.require_cuda(k_all)
-        k_all = k_all.detach().contiguous()
+        k_all = _aligned16(k_all.detach().contiguous())
         if k_all.dim() != 2 or k_all.shape[1] != self.memory.shape[1] or k_all.device != self.memory.device:
             raise ValueError(f"ShardedMemoryMoCo.enqueue: k_all {tuple(k_all.shape)} on {k_all.device} does not match "
                              f"the shard {tuple(self.memory.shape)} on {self.memory.device}")

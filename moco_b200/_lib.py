@@ -182,36 +182,42 @@ class _Counting:
             return rc
         return call
 
+    def _sm_count(self):
+        sms = c_int(0)
+        return sms.value if self._lib.moco_device_info(ctypes.byref(sms), None, None) == 0 else 0
+
     @staticmethod
-    def _head_launches(C, inv_T, flags, dq, logits, f32):
-        """Kernels one head evaluation launches (mirrors the dispatch in csrc/capi.cu)."""
-        simt = bool(flags & NCE_FORCE_SIMT) or C % 64 != 0 or C > 256
-        if simt:
-            return 2                                             # prep + row kernel
+    def _head_plan(N, C, inv_T, flags, dq, logits, f32, sms):
+        """(kernels one head evaluation launches, whether it took the one-sweep path): mirrors the dispatch in
+        csrc/capi.cu.  The tensor-core kernels put one 128-row block of q on each SM, so beyond 128 * #SM rows
+        every flag ends on the CUDA-core kernel."""
+        tc = not (flags & NCE_FORCE_SIMT) and C % 64 == 0 and C <= 256 and (N + 127) // 128 <= sms
+        if not tc:
+            return 2, False                                      # prep + row kernel
         one_pass = (dq and not logits and not (flags & NCE_TWO_PASS)
                     and ((flags & NCE_ONE_PASS) or inv_T <= ONE_PASS_MAX_INV_T))
         if one_pass:                                             # sweep + tail (+ prep for the bf16 copy at C > 128)
-            return 2 + (1 if (C > 128 and f32) else 0)
-        return 5 if dq else 3                                    # prep + stats + combine [+ dq + dq_reduce]
+            return 2 + (1 if (C > 128 and f32) else 0), True
+        return (5 if dq else 3), False                           # prep + stats + combine [+ dq + dq_reduce]
 
-    @classmethod
-    def _wrap_nce(cls, fn):
+    def _wrap_nce(self, fn):
         def call(*a):
             global launches
             rc = fn(*a)
             if rc == 0:
-                launches += cls._head_launches(a[5], a[7], a[16], a[13], a[8], a[2] == MOCO_F32)
+                launches += self._head_plan(a[4], a[5], a[7], a[16], a[13], a[8], a[2] == MOCO_F32, self._sm_count())[0]
             return rc
         return call
 
-    @classmethod
-    def _wrap_step(cls, fn):
+    def _wrap_step(self, fn):
         def call(*a):
             global launches
             rc = fn(*a)
             if rc == 0:
-                n = cls._head_launches(a[7], a[9], a[22], True, False, a[2] == MOCO_F32)
-                fused = n <= 3 and a[7] % 8 == 0 and 256 % (a[7] // 8) == 0      # the tail kernel also enqueues
+                C = a[7]
+                n, one_pass = self._head_plan(a[6], C, a[9], a[22], a[19] is not None, False, a[2] == MOCO_F32,
+                                              self._sm_count())
+                fused = one_pass and C % 8 == 0 and 256 % (C // 8) == 0      # the tail kernel also enqueues
                 launches += n + (0 if (fused or a[12] == 0) else 1)
             return rc
         return call

@@ -49,6 +49,9 @@ static inline void prof_mark(int kernel, int which, cudaStream_t s) {
     if (g_prof_ev[kernel][which]) cudaEventRecord(g_prof_ev[kernel][which], s);
 }
 
+// the kernels' 16-byte vector loads and stores need it; NULL counts as aligned (the caller checks for NULL)
+static bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
+
 }  // namespace moco
 
 using namespace moco;
@@ -111,6 +114,11 @@ static int nce_head(const void* q, const void* k, int qk_dtype, int normalize, c
         set_error("%s: workspace must be 256-byte aligned", who);
         return MOCO_ERR_INVALID;
     }
+    if (misaligned16(q) || misaligned16(queue_bf16) || misaligned16(enq.queue_f32) || misaligned16(enq.k_all)) {
+        set_error("%s: q, the queue and k_all must be 16-byte aligned (q=%p queue=%p queue_f32=%p k_all=%p)", who, q,
+                  queue_bf16, static_cast<const void*>(enq.queue_f32), enq.k_all);
+        return MOCO_ERR_INVALID;
+    }
     NceWorkspace ws = carve_workspace(workspace, N, C);
     if (workspace_bytes < ws.bytes) {
         set_error("%s: workspace too small (%zu < %zu)", who, workspace_bytes, ws.bytes);
@@ -119,8 +127,7 @@ static int nce_head(const void* q, const void* k, int qk_dtype, int normalize, c
     DevInfo d = device_info();
     if (!d.ok) { set_error("%s: no CUDA device", who); return MOCO_ERR_CUDA; }
     const __nv_bfloat16* queue = static_cast<const __nv_bfloat16*>(queue_bf16);
-    const bool aligned = ((reinterpret_cast<uintptr_t>(q) & 15) == 0) && ((reinterpret_cast<uintptr_t>(queue) & 15) == 0);
-    const bool tc_shape = (C % 64 == 0) && C <= 256 && aligned;
+    const bool tc_shape = (C % 64 == 0) && C <= 256;
     const bool want_tc = !(flags & MOCO_NCE_FORCE_SIMT);
     if ((flags & (MOCO_NCE_CTA_PAIR | MOCO_NCE_SINGLE_CTA)) && (!tc_shape || d.major != 9)) {
         set_error("%s: tensor-core path requested but unavailable (C=%d, sm_%d%d)", who, C, d.major, d.minor);
@@ -152,7 +159,7 @@ static int nce_head(const void* q, const void* k, int qk_dtype, int normalize, c
             if (e != cudaSuccess) return cuda_fail("tail kernel", e);
             if (enq.n_all > 0 && !fuse_enq) {
                 e = launch_enqueue(static_cast<__nv_bfloat16*>(enq.queue_bf16), enq.queue_f32, enq.k_all, enq.k_dtype,
-                                   enq.n_all, C, K, enq.index, 0, K, stream);
+                                   enq.n_all, C, K, enq.index, 0, K, stream, enq.index_dev, ws.counters + 2);
                 if (e != cudaSuccess) return cuda_fail("enqueue kernel", e);
             }
             return MOCO_OK;
@@ -160,9 +167,9 @@ static int nce_head(const void* q, const void* k, int qk_dtype, int normalize, c
         if (e != cudaErrorNotSupported) return cuda_fail("one-sweep kernel", e);
         // shape outside the one-sweep kernels' envelope: two-pass below
     }
-    if (normalize || enq.index_dev) {
-        set_error("%s: in-kernel normalisation / device-side ring index need the one-sweep path "
-                  "(C in {64, 128}, gradient requested, no dense logits, inv_T <= %g)", who, (double)MOCO_ONE_PASS_MAX_INV_T);
+    if (normalize) {
+        set_error("%s: in-kernel normalisation needs the one-sweep path (C in {64, 128}, N <= 128 * #SM, gradient "
+                  "requested, no dense logits, inv_T <= %g)", who, (double)MOCO_ONE_PASS_MAX_INV_T);
         return MOCO_ERR_UNSUPPORTED;
     }
     if (!prepped) {
@@ -173,7 +180,8 @@ static int nce_head(const void* q, const void* k, int qk_dtype, int normalize, c
     auto finish = [&]() -> int {                       // the enqueue of moco_nce_step on the non-fused paths
         if (enq.n_all > 0) {
             cudaError_t ee = launch_enqueue(static_cast<__nv_bfloat16*>(enq.queue_bf16), enq.queue_f32, enq.k_all,
-                                            enq.k_dtype, enq.n_all, C, K, enq.index, 0, K, stream);
+                                            enq.k_dtype, enq.n_all, C, K, enq.index, 0, K, stream, enq.index_dev,
+                                            ws.counters + 2);
             if (ee != cudaSuccess) return cuda_fail("enqueue kernel", ee);
         }
         return MOCO_OK;
@@ -288,6 +296,11 @@ int moco_queue_enqueue(void* queue_bf16, float* queue_f32, const void* k_all, in
         set_error("moco_queue_enqueue: n_all (%d) > K (%lld): write order would be ambiguous", n_all, (long long)K);
         return MOCO_ERR_INVALID;
     }
+    if (misaligned16(queue_bf16) || misaligned16(queue_f32) || misaligned16(k_all)) {
+        set_error("moco_queue_enqueue: the queue and k_all must be 16-byte aligned (queue=%p queue_f32=%p k_all=%p)",
+                  queue_bf16, static_cast<void*>(queue_f32), k_all);
+        return MOCO_ERR_INVALID;
+    }
     cudaError_t e = launch_enqueue(static_cast<__nv_bfloat16*>(queue_bf16), queue_f32, k_all, k_dtype, n_all, C, K,
                                    index, 0, K, static_cast<cudaStream_t>(stream_));
     if (e != cudaSuccess) return cuda_fail("enqueue kernel", e);
@@ -303,6 +316,11 @@ int moco_queue_enqueue_shard(void* shard_bf16, float* shard_f32, const void* k_a
     if (!shard_bf16 || !k_all || n_all < 0 || C <= 0 || K <= 0 || index < 0 || index >= K || n_all > K ||
         shard_row0 < 0 || shard_rows <= 0 || shard_row0 + shard_rows > K) {
         set_error("moco_queue_enqueue_shard: bad argument");
+        return MOCO_ERR_INVALID;
+    }
+    if (misaligned16(shard_bf16) || misaligned16(shard_f32) || misaligned16(k_all)) {
+        set_error("moco_queue_enqueue_shard: the shard and k_all must be 16-byte aligned (shard=%p shard_f32=%p k_all=%p)",
+                  shard_bf16, static_cast<void*>(shard_f32), k_all);
         return MOCO_ERR_INVALID;
     }
     cudaError_t e = launch_enqueue(static_cast<__nv_bfloat16*>(shard_bf16), shard_f32, k_all, k_dtype, n_all, C, K,
@@ -507,8 +525,6 @@ int moco_maxpool3x3s2_bwd(const void* dy, const void* taps, void* dx, int N, int
 }
 
 size_t moco_bn_workspace_bytes(void) { return bn_workspace_bytes(); }
-
-static bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
 
 int moco_bn_fwd_train(const void* x, const void* residual, void* y, long long M, int C, const float* gamma,
                       const float* beta, float* running_mean, float* running_var, long long* num_batches_tracked,

@@ -17,7 +17,8 @@ constexpr float kLn2 = 0.6931471805599453f;
 
 // Workspace layout shared by every NCE entry point.
 struct NceWorkspace {
-    unsigned int* counters;   // [4]   (zeroed by the prep / sweep kernel each call)
+    unsigned int* counters;   // [4]   (zeroed by the prep / sweep kernel each call): [0] last-block means,
+                              //       [1] the tail's enqueue release, [2] the separate enqueue's last block
     unsigned long long* cta_times;   // [kMaxCtas][2] %globaltimer at entry / exit of every CTA of the last sweep kernel
     float* lpos;              // [N]   <q_i, k_i> in fp32, natural units
     __nv_bfloat16* q_bf16;    // [N, C] bf16 copy of q (when q arrives as fp32)
@@ -103,9 +104,11 @@ cudaError_t launch_combine_merge(int N, int world, float inv_T, const float2* ms
                                  float* prob_rows, float* loss_prob, const NceWorkspace& ws, cudaStream_t stream);
 cudaError_t launch_bwd_dense(const float* g, const void* k, int k_dtype, const __nv_bfloat16* queue,
                              int N, int C, int K, float inv_T, float* dq, cudaStream_t stream);
+// index_dev != nullptr: the ring position is read from and advanced on the device; `done` is a zeroed workspace
+// counter the kernel uses to find its last block (and re-arms).
 cudaError_t launch_enqueue(__nv_bfloat16* queue_bf16, float* queue_f32, const void* k_all, int k_dtype,
                            int n_all, int C, int64_t K, int64_t index, int64_t shard_row0, int64_t shard_rows,
-                           cudaStream_t stream);
+                           cudaStream_t stream, long long* index_dev = nullptr, unsigned int* done = nullptr);
 cudaError_t launch_f32_to_bf16(const float* src, __nv_bfloat16* dst, size_t n, cudaStream_t stream);
 // bn_*: nullable; the stem's BatchNorm + ReLU applied to each tap (moco_bn_relu_maxpool_fwd_train).
 // eval_scale / eval_shift: nullable; the same with a frozen BatchNorm's folded coefficients (moco_bn_relu_maxpool_eval),

@@ -9,12 +9,34 @@ namespace moco {
 
 // ---------------------------------------------------------------------------
 // enqueue: queue[(index + i) mod K] = k_all[i]; one thread per 8 elements.
+// index_dev != nullptr: the ring position is read from that device int64 instead of `index`, and the last block to
+// finish (counted in `done`, zero on entry and re-armed here) advances it to (index + n_all) mod K once every block
+// has read it -- the same device-side ring as the fused tail kernel's, so a captured graph replays correctly.
 // ---------------------------------------------------------------------------
+__device__ __forceinline__ long long enqueue_ring(long long index, const long long* index_dev) {
+    return index_dev ? *index_dev : index;
+}
+
+__device__ __forceinline__ void enqueue_advance(long long ring, int n_all, long long K, long long* index_dev,
+                                                unsigned int* done) {
+    if (index_dev == nullptr) return;
+    __syncthreads();                                   // every thread of this block has read the ring position
+    if (threadIdx.x == 0) {
+        __threadfence();
+        if (atomicAdd(done, 1u) == gridDim.x - 1) {
+            *index_dev = (ring + n_all) % K;
+            *done = 0u;
+        }
+    }
+}
+
 __global__ void enqueue_kernel(__nv_bfloat16* __restrict__ qb, float* __restrict__ qf,
                                const void* __restrict__ k_all, int k_dtype, int n_all, int C, long long K,
-                               long long index, long long row0, long long nrows) {
+                               long long index, long long row0, long long nrows, long long* index_dev,
+                               unsigned int* done) {
     pdl_launch_dependents();
     pdl_wait();                  // the kernels that read the pre-enqueue queue (this step's head) are complete
+    index = enqueue_ring(index, index_dev);
     const int vec_per_row = C >> 3;
     const long long total = (long long)n_all * vec_per_row;
     for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total;
@@ -44,14 +66,17 @@ __global__ void enqueue_kernel(__nv_bfloat16* __restrict__ qb, float* __restrict
             d[1] = make_float4(f[4], f[5], f[6], f[7]);
         }
     }
+    enqueue_advance(index, n_all, K, index_dev, done);
 }
 
 // scalar variant for C % 8 != 0
 __global__ void enqueue_scalar_kernel(__nv_bfloat16* __restrict__ qb, float* __restrict__ qf,
                                       const void* __restrict__ k_all, int k_dtype, int n_all, int C, long long K,
-                                      long long index, long long row0, long long nrows) {
+                                      long long index, long long row0, long long nrows, long long* index_dev,
+                                      unsigned int* done) {
     pdl_launch_dependents();
     pdl_wait();
+    index = enqueue_ring(index, index_dev);
     const long long total = (long long)n_all * C;
     for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < total;
          t += (long long)gridDim.x * blockDim.x) {
@@ -63,23 +88,26 @@ __global__ void enqueue_scalar_kernel(__nv_bfloat16* __restrict__ qb, float* __r
         qb[(size_t)dst * C + c] = __float2bfloat16_rn(f);
         if (qf) qf[(size_t)dst * C + c] = f;
     }
+    enqueue_advance(index, n_all, K, index_dev, done);
 }
 
 cudaError_t launch_enqueue(__nv_bfloat16* queue_bf16, float* queue_f32, const void* k_all, int k_dtype, int n_all,
-                           int C, int64_t K, int64_t index, int64_t row0, int64_t nrows, cudaStream_t stream) {
+                           int C, int64_t K, int64_t index, int64_t row0, int64_t nrows, cudaStream_t stream,
+                           long long* index_dev, unsigned int* done) {
     if (n_all == 0) return cudaSuccess;
+    if (index_dev != nullptr && done == nullptr) return cudaErrorInvalidValue;
     if ((C & 7) == 0) {
         long long total = (long long)n_all * (C >> 3);
         int blocks = (int)((total + 255) / 256);
         if (blocks > 132 * 8) blocks = 132 * 8;
         return launch_pdl(enqueue_kernel, dim3(blocks), dim3(256), 0, stream, queue_bf16, queue_f32, k_all, k_dtype, n_all, C,
-                          (long long)K, (long long)index, (long long)row0, (long long)nrows);
+                          (long long)K, (long long)index, (long long)row0, (long long)nrows, index_dev, done);
     } else {
         long long total = (long long)n_all * C;
         int blocks = (int)((total + 255) / 256);
         if (blocks > 132 * 8) blocks = 132 * 8;
         return launch_pdl(enqueue_scalar_kernel, dim3(blocks), dim3(256), 0, stream, queue_bf16, queue_f32, k_all, k_dtype,
-                          n_all, C, (long long)K, (long long)index, (long long)row0, (long long)nrows);
+                          n_all, C, (long long)K, (long long)index, (long long)row0, (long long)nrows, index_dev, done);
     }
     return cudaGetLastError();
 }

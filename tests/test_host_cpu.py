@@ -328,3 +328,82 @@ def test_bn_and_pool_entries_validate_their_arguments_without_a_gpu():
     assert rc == -1 and b"moco_bn_bwd" in lib.moco_last_error()
     assert lib.moco_maxpool3x3s2_fwd(None, None, None, 1, 8, 8, 64, None) == -1
     assert lib.moco_maxpool3x3s2_bwd(None, None, None, 1, 8, 8, 64, None) == -1
+
+
+# Addresses that are never dereferenced: every call below must return before it touches the device.
+_A, _WS = 0x7f0000001000, 0x7f0000100000          # 16-byte / 256-byte aligned
+
+
+@pytest.mark.parametrize("bad", ["q", "queue"])
+def test_nce_fwd_rejects_misaligned_operands_without_a_gpu(bad):
+    """q and the queue are read with 16-byte vector loads (TMA / uint4 rows): a contiguous view at an odd storage
+    offset must be refused before any device access, not handed to a kernel that would fault."""
+    from moco_b200 import _lib
+    lib = _lib.load()
+    ptr = {"q": _A, "queue": _A + 0x10000}
+    ptr[bad] += 8
+    args = lambda ws_bytes: (ptr["q"], _A + 0x20000, _lib.MOCO_BF16, ptr["queue"], 4, 64, 16, 1 / 0.07, None,
+                             _A + 0x30000, _A + 0x30100, _A + 0x30200, _A + 0x30300, _A + 0x40000, _WS, ws_bytes, 0, None)
+    rc = lib.moco_nce_fwd(*args(1 << 30))
+    assert rc == -1 and b"16-byte aligned" in lib.moco_last_error(), lib.moco_last_error()
+    ptr[bad] -= 8                                 # control: aligned, the next check (workspace size) answers
+    assert lib.moco_nce_fwd(*args(0)) == -3
+
+
+@pytest.mark.parametrize("bad", ["q", "queue", "queue_f32", "k_all"])
+def test_nce_step_rejects_misaligned_operands_without_a_gpu(bad):
+    from moco_b200 import _lib
+    lib = _lib.load()
+    ptr = {"q": _A, "queue": _A + 0x10000, "queue_f32": _A + 0x20000, "k_all": _A + 0x50000}
+    ptr[bad] += 4
+    args = lambda ws_bytes: (ptr["q"], _A + 0x60000, _lib.MOCO_F32, 0, ptr["queue"], ptr["queue_f32"], 4, 64, 16,
+                             1 / 0.07, ptr["k_all"], _lib.MOCO_F32, 4, 3, None, _A + 0x30000, _A + 0x30100,
+                             _A + 0x30200, _A + 0x30300, _A + 0x40000, _WS, ws_bytes, 0, None)
+    rc = lib.moco_nce_step(*args(1 << 30))
+    assert rc == -1 and b"16-byte aligned" in lib.moco_last_error(), lib.moco_last_error()
+    ptr[bad] -= 4
+    assert lib.moco_nce_step(*args(0)) == -3
+
+
+@pytest.mark.parametrize("bad", ["queue", "queue_f32", "k_all"])
+def test_enqueue_entries_reject_misaligned_operands_without_a_gpu(bad):
+    """enqueue_kernel reads k_all and writes both queue copies 16 bytes at a time."""
+    from moco_b200 import _lib
+    lib = _lib.load()
+    ptr = {"queue": _A, "queue_f32": _A + 0x10000, "k_all": _A + 0x20000}
+    ptr[bad] += 2
+    rc = lib.moco_queue_enqueue(ptr["queue"], ptr["queue_f32"], ptr["k_all"], _lib.MOCO_BF16, 4, 64, 16, 3, None)
+    assert rc == -1 and b"moco_queue_enqueue: the queue and k_all must be 16-byte aligned" in lib.moco_last_error()
+    rc = lib.moco_queue_enqueue_shard(ptr["queue"], ptr["queue_f32"], ptr["k_all"], _lib.MOCO_BF16, 4, 64, 16, 3, 0, 8,
+                                      None)
+    assert rc == -1 and b"moco_queue_enqueue_shard: the shard and k_all must be 16-byte aligned" in lib.moco_last_error()
+
+
+def test_memory_moco_copies_a_misaligned_view_before_the_kernels_see_it():
+    """A contiguous view at an odd storage offset passes .contiguous() unchanged; MemoryMoCo copies it instead."""
+    from moco_b200.NCE.Contrast import _aligned16
+    base = torch.zeros(1 + 4 * 64)
+    view = base[1:].view(4, 64)
+    assert view.is_contiguous() and view.data_ptr() % 16 != 0
+    fixed = _aligned16(view)
+    assert fixed.data_ptr() % 16 == 0 and torch.equal(fixed, view)
+    ok = torch.zeros(4, 64)
+    assert _aligned16(ok) is ok
+
+
+@pytest.mark.parametrize("N,C,flags,dq,logits,f32,expect", [
+    (256, 128, 0, True, False, True, (2, True)),          # one sweep + tail
+    (256, 256, 0, True, False, True, (3, True)),          # + the bf16 copy of q
+    (256, 128, 512, True, False, False, (5, False)),      # prep, stats, combine, dq, dq_reduce
+    (256, 128, 0, False, False, False, (3, False)),       # no gradient: the statistics pass only
+    (256, 128, 0, True, True, False, (5, False)),         # dense logits
+    (256, 100, 0, True, False, False, (2, False)),        # C % 64 != 0: prep + CUDA-core rows
+    (256, 128, 1, True, False, False, (2, False)),        # FORCE_SIMT
+    (16896, 128, 0, True, False, False, (2, True)),       # 132 blocks of 128 rows: still the one sweep
+    (16897, 128, 0, True, False, False, (2, False)),      # more q blocks than SMs: the CUDA-core kernel
+    (16897, 256, 0, True, False, True, (2, False)),       # (its prep doubles as the bf16 copy)
+    (16897, 128, 512, True, False, False, (2, False)),
+])
+def test_head_launch_count_follows_the_dispatch(N, C, flags, dq, logits, f32, expect):
+    from moco_b200 import _lib
+    assert _lib._Counting._head_plan(N, C, 1 / 0.07, flags, dq, logits, f32, 132) == expect
