@@ -328,6 +328,13 @@ int moco_bn_add_relu_fwd_train(const void* x, const void* residual, void* y, voi
 int moco_bn_add_relu_bwd(const void* dy, const void* x, const void* residual, const void* mask, long long M, int C,
                          const moco_bn_layer* bn, const moco_bn_layer* shortcut_or_null, void* dx,
                          void* dresidual_or_null, void* workspace, size_t workspace_bytes, void* stream);
+/* moco_bn_add_relu_bwd2: moco_bn_add_relu_bwd with y's gradient arriving in two parts, dy and dy2 (bf16 [M, C]): the
+ * input of the next block feeds both its first convolution and its residual branch.  Both passes read both and use
+ * bf16(dy + dy2) (fp32 add, one rounding -- what a separate bf16 add would store), which is never written; the
+ * results are bit-identical to that add followed by moco_bn_add_relu_bwd.  Two launches. */
+int moco_bn_add_relu_bwd2(const void* dy, const void* dy2, const void* x, const void* residual, const void* mask,
+                          long long M, int C, const moco_bn_layer* bn, const moco_bn_layer* shortcut_or_null, void* dx,
+                          void* dresidual_or_null, void* workspace, size_t workspace_bytes, void* stream);
 
 /* The stem's BatchNorm + ReLU followed by its 3x3 / stride 2 / pad 1 max pooling, without writing the BatchNorm's
  * output: bit-identical to moco_bn_fwd_train (relu = 1, no residual) + moco_maxpool3x3s2_fwd.  The statistics pass,
@@ -394,10 +401,15 @@ int moco_crop_s2d_bf16(const void* src, int src_dtype, long long src_image_strid
  * (first maximum in kh-then-kw order, NaN wins -- torch's rule), written by the
  * forward and consumed by the backward, which adds dy into the winning input
  * element of every window (gather over the <= 4 windows of a pixel: no atomics,
- * deterministic).  One launch each.
+ * deterministic, fp32 sums in increasing (oh, ow) order).  N <= 65535.  One launch each.
+ * moco_maxpool3x3s2_bwd2: the backward with the pooled output's gradient in two parts, dy and dy2 (the stem's output
+ * feeds the first block's convolution and its residual branch): each window's gradient is bf16(dy + dy2), the value a
+ * separate bf16 add would store, never written; bit-identical to that add followed by moco_maxpool3x3s2_bwd.
  * ---------------------------------------------------------------------- */
 int moco_maxpool3x3s2_fwd(const void* x, void* y, void* taps_u8, int N, int H, int W, int C, void* stream);
 int moco_maxpool3x3s2_bwd(const void* dy, const void* taps_u8, void* dx, int N, int H, int W, int C, void* stream);
+int moco_maxpool3x3s2_bwd2(const void* dy, const void* dy2, const void* taps_u8, void* dx, int N, int H, int W, int C,
+                           void* stream);
 
 /* ------------------------------------------------------------------------
  * Input path (SURVEY.md 8 f3): one crop of the [N, C_total, H, W] batch ->

@@ -11,6 +11,9 @@ shortcut_bn=...)``) the shortcut's BatchNorm runs inside the same passes, so nei
 between the two BatchNorms is ever written.  The stem's BatchNorm + ReLU and its max pool (``forward_maxpool``) run
 as ``moco_bn_relu_maxpool_fwd_train``: the pool applies the BatchNorm to each tap, so the stem's full-resolution
 activation is never written.
+A block's input has two consumers; ``hand_over`` (called by the encoders' blocks in front of the residual branch)
+passes that branch's gradient to the producer's backward, which adds it to the other one inside its own kernels
+(``moco_bn_add_relu_bwd2`` / ``moco_maxpool3x3s2_bwd2``) instead of autograd adding them in a pass of its own.
 The results are bit-identical to the separate calls.
 A FROZEN module (``frozen = True``, set by :meth:`moco_b200.encoders.MoCoResNet.freeze`) in eval mode under
 ``torch.no_grad()`` -- the linear probe's encoder -- runs the eval kernels instead: the running statistics are folded
@@ -66,6 +69,22 @@ def _workspace(device):
 def _rows_ok(t, like=None):
     return (t.is_cuda and t.dtype == torch.bfloat16 and t.dim() == 4 and t.numel() > 0
             and t.is_contiguous(memory_format=torch.channels_last) and (like is None or t.shape == like.shape))
+
+
+def _grad_rows(g):
+    if g.dtype != torch.bfloat16:
+        g = g.to(torch.bfloat16)
+    return g.contiguous(memory_format=torch.channels_last)
+
+
+def _take_handed(ctx):
+    """The gradient a :class:`_HandOverFn` left on this node during the current backward (None without one), taken
+    exactly once, so that a second backward through a retained graph sees only what its own hand-over leaves."""
+    g = getattr(ctx, "handed", None)
+    if g is None:
+        return None
+    ctx.handed = None
+    return _grad_rows(g)
 
 
 class _BatchNormActFn(torch.autograd.Function):
@@ -174,9 +193,8 @@ class _BatchNormAddReluFn(torch.autograd.Function):
         lib = _lib.load()
         N, C, H, W = x.shape
         M = N * H * W
-        if dy.dtype != torch.bfloat16:
-            dy = dy.to(torch.bfloat16)
-        dy = dy.contiguous(memory_format=torch.channels_last)
+        dy = _grad_rows(dy)
+        dy2 = _take_handed(ctx)          # y's other consumer's gradient: summed inside both passes
         dx = torch.empty_like(x)
         f32 = lambda: torch.empty(C, dtype=torch.float32, device=x.device)
         dgamma, dbeta = f32(), f32()
@@ -189,13 +207,21 @@ class _BatchNormAddReluFn(torch.autograd.Function):
         else:
             dres = torch.empty_like(x) if ctx.needs_input_grad[1] else None
         ws = _workspace(x.device)
-        # algorithmic bytes: reduce reads dy, x, mask (+ shortcut input); apply reads the same and writes dx (+ d residual)
-        nbytes = M * C * 2 * (5 + (dres is not None) + 2 * (sc is not None)) + 2 * (M * C // 8)
-        code = _timed("bn_bwd", nbytes, lambda: lib.moco_bn_add_relu_bwd(
-            dy.data_ptr(), x.data_ptr(), residual.data_ptr() if residual is not None else None, mask.data_ptr(), M, C,
-            bn, sc, dx.data_ptr(), dres.data_ptr() if dres is not None else None, ws.data_ptr(), ws.numel(),
-            _lib.cur_stream()))
-        _lib.check(code, "moco_bn_add_relu_bwd")
+        # algorithmic bytes: reduce reads dy (+ dy2), x, mask (+ shortcut input); apply reads the same and writes dx
+        # (+ d residual)
+        nbytes = (M * C * 2 * (5 + (dres is not None) + 2 * (sc is not None) + 2 * (dy2 is not None))
+                  + 2 * (M * C // 8))
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        if dy2 is None:
+            code = _timed("bn_bwd", nbytes, lambda: lib.moco_bn_add_relu_bwd(
+                dy.data_ptr(), x.data_ptr(), ptr(residual), mask.data_ptr(), M, C, bn, sc, dx.data_ptr(), ptr(dres),
+                ws.data_ptr(), ws.numel(), _lib.cur_stream()))
+            _lib.check(code, "moco_bn_add_relu_bwd")
+        else:
+            code = _timed("bn_bwd", nbytes, lambda: lib.moco_bn_add_relu_bwd2(
+                dy.data_ptr(), dy2.data_ptr(), x.data_ptr(), ptr(residual), mask.data_ptr(), M, C, bn, sc,
+                dx.data_ptr(), ptr(dres), ws.data_ptr(), ws.numel(), _lib.cur_stream()))
+            _lib.check(code, "moco_bn_add_relu_bwd2")
         return dx, dres, dgamma, dbeta, sc_dgamma, sc_dbeta, None, None, None
 
 
@@ -228,14 +254,17 @@ class _BatchNormReluMaxPoolFn(torch.autograd.Function):
         x, taps, weight, bias, mean, invstd = ctx.saved_tensors
         lib = _lib.load()
         N, C, H, W = x.shape
-        if dy.dtype != torch.bfloat16:
-            dy = dy.to(torch.bfloat16)
-        dy = dy.contiguous(memory_format=torch.channels_last)
+        dy = _grad_rows(dy)
+        dy2 = _take_handed(ctx)          # the pooled output's other consumer's gradient: summed inside the gather
         # Rebuilding the pool's input gradient inside the BatchNorm's two passes (a <= 4-window gather per element)
         # measured slower than writing it once and streaming it: the pool's backward, then the BatchNorm's.
         g = torch.empty_like(x)
-        _lib.check(lib.moco_maxpool3x3s2_bwd(dy.data_ptr(), taps.data_ptr(), g.data_ptr(), N, H, W, C, _lib.cur_stream()),
-                   "moco_maxpool3x3s2_bwd")
+        if dy2 is None:
+            _lib.check(lib.moco_maxpool3x3s2_bwd(dy.data_ptr(), taps.data_ptr(), g.data_ptr(), N, H, W, C,
+                                                 _lib.cur_stream()), "moco_maxpool3x3s2_bwd")
+        else:
+            _lib.check(lib.moco_maxpool3x3s2_bwd2(dy.data_ptr(), dy2.data_ptr(), taps.data_ptr(), g.data_ptr(), N, H, W,
+                                                  C, _lib.cur_stream()), "moco_maxpool3x3s2_bwd2")
         dx = torch.empty_like(x)
         dgamma = torch.empty(C, dtype=torch.float32, device=x.device)
         dbeta = torch.empty_like(dgamma)
@@ -247,6 +276,37 @@ class _BatchNormReluMaxPoolFn(torch.autograd.Function):
             ws.numel(), _lib.cur_stream()))
         _lib.check(code, "moco_bn_bwd")
         return dx, dgamma, dbeta, None
+
+
+class _HandOverFn(torch.autograd.Function):
+    """Identity in front of the second consumer of a block's input.  The input has two consumers (the first
+    convolution, and the residual branch: bn3's residual or the shortcut convolution), so autograd would add their two
+    bf16 gradients in a separate pass before the producer's backward reads the sum twice.  Instead the backward leaves
+    this branch's gradient on the producer's node and returns None; the producer (a _BatchNormAddReluFn or the stem's
+    _BatchNormReluMaxPoolFn) receives the other gradient from autograd and adds the two inside its own kernels,
+    rounded to bf16 once as autograd's add would -- the sum is never written."""
+
+    @staticmethod
+    def forward(ctx, x, producer):
+        ctx.producer = producer
+        return x
+
+    @staticmethod
+    def backward(ctx, g):
+        ctx.producer.handed = g          # this node runs before the producer's: taken by its backward (_take_handed)
+        return None, None
+
+
+def hand_over(x):
+    """``x`` for a second consumer of ``x``; through :class:`_HandOverFn` when x's producer sums its gradients in its
+    own kernels.  Anything else -- no grad, set_fused(False), a producer that is not one of those Functions -- gets x
+    itself, so autograd adds the gradients as usual."""
+    if not (_enabled and torch.is_grad_enabled() and x.requires_grad):
+        return x
+    node = x.grad_fn
+    if not isinstance(node, (_BatchNormAddReluFn._backward_cls, _BatchNormReluMaxPoolFn._backward_cls)):
+        return x
+    return _HandOverFn.apply(x, node)
 
 
 class BatchNormAct2d(nn.BatchNorm2d):

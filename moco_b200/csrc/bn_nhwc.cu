@@ -17,6 +17,8 @@
 //   bn_bwd_reduce_kernel reads dy, x (+ y)   -> sum(g), sum(g * x^) = dbeta, dgamma     4 (6) B / element
 //   bn_bwd_apply_kernel  reads dy, x (+ y), writes dx (+ d residual)                    6 (10) B / element
 // where g = dy masked by the ReLU (the mask is recomputed from x when there is no residual, read from y otherwise).
+// A block output's gradient may arrive in two parts (the next block's first convolution and its residual branch):
+// both backward passes then read dy and dy2 and use bf16(dy + dy2), +2 B / element each (kSum, moco_bn_add_relu_bwd2).
 //
 // Reductions: a CTA owns a 64-channel slab (128 contiguous bytes of every row = one 16-byte vector per lane of an
 // 8-lane group) and a contiguous range of rows, 32 rows per pass, 4 or 8 passes in flight (see the table of measured
@@ -44,6 +46,7 @@ constexpr int kBnApplyUnroll = 8, kBnApplyCtas = 2;
 constexpr int kBnBwdReduceUnroll = 4, kBnBwdReduceCtas = 2;
 constexpr int kBnBwdApplyUnroll = 2, kBnBwdApplyCtas = 3;
 constexpr int kBnBwdApplyScUnroll = 2, kBnBwdApplyScCtas = 2;   // with the shortcut BN: 48 coefficients per thread
+constexpr int kBnBwdApplySumUnroll = 2, kBnBwdApplySumCtas = 2; // with a second gradient (dy2): spills at 3 CTAs / SM
 constexpr int kBnSms = 132;
 constexpr int kBnMaxCtas = kBnSms * 4;               // workspace sizing: no reduction grid is larger
 
@@ -308,8 +311,18 @@ bn_apply_kernel(const BnApplyArgs a) {
 // how the ReLU mask of the backward is obtained
 enum { kMaskNone = 0, kMaskFromY = 1, kMaskFromX = 2, kMaskFromBits = 3 };
 
+// kSum: the incoming gradient is the sum of two, dy + dy2, rounded to bf16 once before any other use -- what autograd's
+// bf16 add of the two branch gradients of a block's input would have stored (fp32 add, one rounding); never written
+__device__ __forceinline__ void sum_grads(float* d, const uint4& u2) {
+    float d2[8];
+    unpack8(u2, d2);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) d[k] = __bfloat162float(__float2bfloat16_rn(__fadd_rn(d[k], d2[k])));
+}
+
 struct BnBwdReduceArgs {
     const uint4* dy;
+    const uint4* dy2;                // kSum only: the second gradient of y
     const uint4* x;
     const uint4* y;                  // kMaskFromY only
     const uint8_t* mbits;            // kMaskFromBits only: the forward's mask bytes
@@ -339,7 +352,7 @@ __device__ __forceinline__ bool mask_on(int mode, float y, unsigned int bits, in
 
 // kShortcut: the block's bn3 and the shortcut BN of a downsample block, both fed by the same masked gradient g: a
 // third sum, g * (x2 - mean2), taken in the same row / slab plan and per-thread order as the shortcut's own reduction.
-template <int kUnroll, int kCtas, bool kShortcut>
+template <int kUnroll, int kCtas, bool kShortcut, bool kSum>
 __global__ void __launch_bounds__(kBnThreads, kCtas)
 bn_bwd_reduce_kernel(const BnBwdReduceArgs a) {
     constexpr int S = kShortcut ? 3 : 2;
@@ -369,7 +382,7 @@ bn_bwd_reduce_kernel(const BnBwdReduceArgs a) {
     const long long p0 = (long long)r * a.ppc;
     const long long p1 = (p0 + a.ppc < a.passes) ? p0 + a.ppc : a.passes;
     for (long long p = p0; p < p1; p += kUnroll) {
-        uint4 ud[kUnroll], ux[kUnroll], uy[kUnroll], u2[kShortcut ? kUnroll : 1];
+        uint4 ud[kUnroll], ux[kUnroll], uy[kUnroll], u2[kShortcut ? kUnroll : 1], us[kSum ? kUnroll : 1];
         unsigned int mb[kUnroll];
         bool live[kUnroll];
 #pragma unroll
@@ -378,10 +391,12 @@ bn_bwd_reduce_kernel(const BnBwdReduceArgs a) {
             live[t] = (p + t < p1) && row < a.M;
             ud[t] = ux[t] = uy[t] = make_uint4(0u, 0u, 0u, 0u);
             if constexpr (kShortcut) u2[t] = make_uint4(0u, 0u, 0u, 0u);
+            if constexpr (kSum) us[t] = make_uint4(0u, 0u, 0u, 0u);
             mb[t] = 0u;
             if (live[t]) {
                 const long long j = row * vec_per_row + colv;
                 ud[t] = __ldg(a.dy + j);
+                if constexpr (kSum) us[t] = __ldg(a.dy2 + j);
                 ux[t] = __ldg(a.x + j);
                 if (mode == kMaskFromY) uy[t] = __ldg(a.y + j);
                 if (mode == kMaskFromBits) mb[t] = __ldg(a.mbits + j);
@@ -393,6 +408,7 @@ bn_bwd_reduce_kernel(const BnBwdReduceArgs a) {
             if (live[t]) {
                 float d[8], f[8], yy[8], f2[kShortcut ? 8 : 1];
                 unpack8(ud[t], d);
+                if constexpr (kSum) sum_grads(d, us[t]);
                 unpack8(ux[t], f);
                 unpack8(uy[t], yy);
                 if constexpr (kShortcut) unpack8(u2[t], f2);
@@ -422,6 +438,7 @@ bn_bwd_reduce_kernel(const BnBwdReduceArgs a) {
 
 struct BnBwdApplyArgs {
     const uint4* dy;
+    const uint4* dy2;                // kSum only
     const uint4* x;
     const uint4* y;                  // kMaskFromY only
     const uint8_t* mbits;            // kMaskFromBits only
@@ -455,7 +472,7 @@ __device__ __forceinline__ void bwd_coefs(float gamma, float mu, float is, float
     cD = fmaf(-cB, mu, -k1 * m1);
 }
 
-template <int kUnroll, int kCtas, bool kShortcut>
+template <int kUnroll, int kCtas, bool kShortcut, bool kSum>
 __global__ void __launch_bounds__(kBnThreads, kCtas)
 bn_bwd_apply_kernel(const BnBwdApplyArgs a) {
     const int lanes = a.C >> 3;
@@ -476,16 +493,18 @@ bn_bwd_apply_kernel(const BnBwdApplyArgs a) {
     }
     const long long stride = (long long)gridDim.x * kBnThreads;
     for (long long i = (long long)blockIdx.x * kBnThreads + threadIdx.x; i < a.V; i += stride * kUnroll) {
-        uint4 ud[kUnroll], ux[kUnroll], uy[kUnroll], u2[kShortcut ? kUnroll : 1];
+        uint4 ud[kUnroll], ux[kUnroll], uy[kUnroll], u2[kShortcut ? kUnroll : 1], us[kSum ? kUnroll : 1];
         unsigned int mb[kUnroll];
 #pragma unroll
         for (int t = 0; t < kUnroll; ++t) {
             const long long j = i + t * stride;
             ud[t] = ux[t] = uy[t] = make_uint4(0u, 0u, 0u, 0u);
             if constexpr (kShortcut) u2[t] = make_uint4(0u, 0u, 0u, 0u);
+            if constexpr (kSum) us[t] = make_uint4(0u, 0u, 0u, 0u);
             mb[t] = 0u;
             if (j < a.V) {
                 ud[t] = __ldg(a.dy + j);
+                if constexpr (kSum) us[t] = __ldg(a.dy2 + j);
                 ux[t] = __ldg(a.x + j);
                 if (mode == kMaskFromY) uy[t] = __ldg(a.y + j);
                 if (mode == kMaskFromBits) mb[t] = __ldg(a.mbits + j);
@@ -498,6 +517,7 @@ bn_bwd_apply_kernel(const BnBwdApplyArgs a) {
             if (j < a.V) {
                 float d[8], f[8], yy[8], o[8];
                 unpack8(ud[t], d);
+                if constexpr (kSum) sum_grads(d, us[t]);
                 unpack8(ux[t], f);
                 unpack8(uy[t], yy);
 #pragma unroll
@@ -689,15 +709,15 @@ static cudaError_t run_apply(BnApplyArgs& p, cudaStream_t stream) {
     bn_apply_kernel<U, CT, SC><<<bn_apply_grid(p.V, U, CT), kBnThreads, 0, stream>>>(p);
     return cudaGetLastError();
 }
-template <int U, int CT, bool SC>
+template <int U, int CT, bool SC, bool SUM = false>
 static cudaError_t run_bwd_reduce(BnBwdReduceArgs& s, cudaStream_t stream) {
     bn_reduce_plan(s.M, s.C, U, CT, &s.passes, &s.ppc, &s.R);
-    bn_bwd_reduce_kernel<U, CT, SC><<<dim3(s.C / kBnSlab, s.R), kBnThreads, 0, stream>>>(s);
+    bn_bwd_reduce_kernel<U, CT, SC, SUM><<<dim3(s.C / kBnSlab, s.R), kBnThreads, 0, stream>>>(s);
     return cudaGetLastError();
 }
-template <int U, int CT, bool SC>
+template <int U, int CT, bool SC, bool SUM = false>
 static cudaError_t run_bwd_apply(BnBwdApplyArgs& p, cudaStream_t stream) {
-    bn_bwd_apply_kernel<U, CT, SC><<<bn_apply_grid(p.V, U, CT), kBnThreads, 0, stream>>>(p);
+    bn_bwd_apply_kernel<U, CT, SC, SUM><<<bn_apply_grid(p.V, U, CT), kBnThreads, 0, stream>>>(p);
     return cudaGetLastError();
 }
 
@@ -770,12 +790,33 @@ cudaError_t launch_bn_add_relu_fwd(const void* x, const void* res, void* y, void
     return run_apply<kBnApplyUnroll, kBnApplyCtas, true>(p, stream);
 }
 
-cudaError_t launch_bn_add_relu_bwd(const void* dy, const void* x, const void* res, const void* mask, long long M, int C,
-                                   const BnLayer& bn, const BnLayer* sc, void* dx, void* dres, void* ws,
-                                   cudaStream_t stream) {
+template <bool SUM>
+static cudaError_t add_relu_bwd(BnBwdReduceArgs& s, BnBwdApplyArgs& p, const BnLayer* sc, void* dres,
+                                cudaStream_t stream) {
+    cudaError_t e;
+    if (sc == nullptr) {
+        p.dres = static_cast<uint4*>(dres);
+        e = run_bwd_reduce<kBnBwdReduceUnroll, kBnBwdReduceCtas, false, SUM>(s, stream);
+        if (e != cudaSuccess) return e;
+        if constexpr (SUM) return run_bwd_apply<kBnBwdApplySumUnroll, kBnBwdApplySumCtas, false, true>(p, stream);
+        return run_bwd_apply<kBnBwdApplyUnroll, kBnBwdApplyCtas, false, false>(p, stream);
+    }
+    s.x2 = p.x2;
+    s.mean2 = sc->save_mean; s.invstd2 = sc->save_invstd;
+    s.sum_dy2 = sc->dbeta; s.sum_dy_xhat2 = sc->dgamma;
+    e = run_bwd_reduce<kBnBwdReduceUnroll, kBnBwdReduceCtas, true, SUM>(s, stream);
+    if (e != cudaSuccess) return e;
+    p.dx2 = static_cast<uint4*>(dres);
+    p.mean2 = sc->save_mean; p.invstd2 = sc->save_invstd; p.gamma2 = sc->gamma; p.sum_dy_xhat2 = sc->dgamma;
+    return run_bwd_apply<kBnBwdApplyScUnroll, kBnBwdApplyScCtas, true, SUM>(p, stream);
+}
+
+cudaError_t launch_bn_add_relu_bwd(const void* dy, const void* dy2, const void* x, const void* res, const void* mask,
+                                   long long M, int C, const BnLayer& bn, const BnLayer* sc, void* dx, void* dres,
+                                   void* ws, cudaStream_t stream) {
     if (!bn_shape_ok(M, C)) return cudaErrorNotSupported;
     BnBwdReduceArgs s{};
-    s.dy = static_cast<const uint4*>(dy); s.x = static_cast<const uint4*>(x);
+    s.dy = static_cast<const uint4*>(dy); s.dy2 = static_cast<const uint4*>(dy2); s.x = static_cast<const uint4*>(x);
     s.mbits = static_cast<const uint8_t*>(mask);
     s.M = M; s.C = C; s.mask = kMaskFromBits;
     s.counters = static_cast<unsigned int*>(ws);
@@ -783,25 +824,12 @@ cudaError_t launch_bn_add_relu_bwd(const void* dy, const void* x, const void* re
     s.mean = bn.save_mean; s.invstd = bn.save_invstd; s.gamma = bn.gamma;
     s.sum_dy = bn.dbeta; s.sum_dy_xhat = bn.dgamma;
     BnBwdApplyArgs p{};
-    p.dy = s.dy; p.x = s.x; p.mbits = s.mbits; p.dx = static_cast<uint4*>(dx);
+    p.dy = s.dy; p.dy2 = s.dy2; p.x = s.x; p.mbits = s.mbits; p.dx = static_cast<uint4*>(dx);
+    p.x2 = static_cast<const uint4*>(res);
     p.V = M * (C >> 3); p.C = C; p.mask = kMaskFromBits; p.inv_m = (float)(1.0 / (double)M);
     p.mean = bn.save_mean; p.invstd = bn.save_invstd; p.gamma = bn.gamma;
     p.sum_dy = bn.dbeta; p.sum_dy_xhat = bn.dgamma;
-    cudaError_t e;
-    if (sc == nullptr) {
-        p.dres = static_cast<uint4*>(dres);
-        e = run_bwd_reduce<kBnBwdReduceUnroll, kBnBwdReduceCtas, false>(s, stream);
-        if (e != cudaSuccess) return e;
-        return run_bwd_apply<kBnBwdApplyUnroll, kBnBwdApplyCtas, false>(p, stream);
-    }
-    s.x2 = static_cast<const uint4*>(res);
-    s.mean2 = sc->save_mean; s.invstd2 = sc->save_invstd;
-    s.sum_dy2 = sc->dbeta; s.sum_dy_xhat2 = sc->dgamma;
-    e = run_bwd_reduce<kBnBwdReduceUnroll, kBnBwdReduceCtas, true>(s, stream);
-    if (e != cudaSuccess) return e;
-    p.x2 = s.x2; p.dx2 = static_cast<uint4*>(dres);
-    p.mean2 = sc->save_mean; p.invstd2 = sc->save_invstd; p.gamma2 = sc->gamma; p.sum_dy_xhat2 = sc->dgamma;
-    return run_bwd_apply<kBnBwdApplyScUnroll, kBnBwdApplyScCtas, true>(p, stream);
+    return dy2 != nullptr ? add_relu_bwd<true>(s, p, sc, dres, stream) : add_relu_bwd<false>(s, p, sc, dres, stream);
 }
 
 cudaError_t launch_bn_relu_maxpool_fwd(const void* x, void* y, void* taps, int N, int H, int W, int C, const BnLayer& bn,

@@ -518,8 +518,22 @@ int moco_maxpool3x3s2_bwd(const void* dy, const void* taps, void* dx, int N, int
         set_error("moco_maxpool3x3s2_bwd: null or misaligned pointer");
         return MOCO_ERR_INVALID;
     }
-    cudaError_t e = launch_maxpool_bwd(dy, taps, dx, N, H, W, C, static_cast<cudaStream_t>(stream_));
+    cudaError_t e = launch_maxpool_bwd(dy, nullptr, taps, dx, N, H, W, C, static_cast<cudaStream_t>(stream_));
     if (e == cudaErrorNotSupported) { set_error("moco_maxpool3x3s2_bwd: needs N, H, W >= 1 and C %% 8 == 0 (C=%d)", C); return MOCO_ERR_UNSUPPORTED; }
+    if (e != cudaSuccess) return cuda_fail("max-pool backward kernel", e);
+    return MOCO_OK;
+}
+
+int moco_maxpool3x3s2_bwd2(const void* dy, const void* dy2, const void* taps, void* dx, int N, int H, int W, int C,
+                           void* stream_) {
+    g_err[0] = 0;
+    if (!dy || !dy2 || !dx || !taps || misaligned16(dy) || misaligned16(dy2) || misaligned16(dx) ||
+        (reinterpret_cast<uintptr_t>(taps) & 7)) {
+        set_error("moco_maxpool3x3s2_bwd2: null or misaligned pointer");
+        return MOCO_ERR_INVALID;
+    }
+    cudaError_t e = launch_maxpool_bwd(dy, dy2, taps, dx, N, H, W, C, static_cast<cudaStream_t>(stream_));
+    if (e == cudaErrorNotSupported) { set_error("moco_maxpool3x3s2_bwd2: needs N, H, W >= 1 and C %% 8 == 0 (C=%d)", C); return MOCO_ERR_UNSUPPORTED; }
     if (e != cudaSuccess) return cuda_fail("max-pool backward kernel", e);
     return MOCO_OK;
 }
@@ -610,10 +624,33 @@ int moco_bn_add_relu_bwd(const void* dy, const void* x, const void* residual, co
         return MOCO_ERR_INVALID;
     }
     if (workspace_bytes < bn_workspace_bytes()) { set_error("moco_bn_add_relu_bwd: workspace too small"); return MOCO_ERR_WORKSPACE; }
-    cudaError_t e = launch_bn_add_relu_bwd(dy, x, residual, mask, M, C, *bn, shortcut, dx, dresidual, workspace,
-                                           static_cast<cudaStream_t>(stream_));
+    cudaError_t e = launch_bn_add_relu_bwd(dy, nullptr, x, residual, mask, M, C, *bn, shortcut, dx, dresidual,
+                                           workspace, static_cast<cudaStream_t>(stream_));
     if (e == cudaErrorNotSupported) {
         set_error("moco_bn_add_relu_bwd: needs M >= 1 and C a power of two in [64, 2048] (M=%lld C=%d)", M, C);
+        return MOCO_ERR_UNSUPPORTED;
+    }
+    if (e != cudaSuccess) return cuda_fail("batch-norm backward kernels", e);
+    return MOCO_OK;
+}
+
+int moco_bn_add_relu_bwd2(const void* dy, const void* dy2, const void* x, const void* residual, const void* mask,
+                          long long M, int C, const moco_bn_layer* bn, const moco_bn_layer* shortcut, void* dx,
+                          void* dresidual, void* workspace, size_t workspace_bytes, void* stream_) {
+    g_err[0] = 0;
+    if (!dy || !dy2 || !x || !mask || !dx || !workspace || !bn_layer_bwd_ok(bn) ||
+        (shortcut && (!bn_layer_bwd_ok(shortcut) || !residual || !dresidual)) || misaligned16(dy) ||
+        misaligned16(dy2) || misaligned16(x) || misaligned16(residual) || misaligned16(dx) || misaligned16(dresidual) ||
+        misaligned16(workspace)) {
+        set_error("moco_bn_add_relu_bwd2: bad argument (null / misaligned pointer; residual and dresidual are required "
+                  "with a shortcut BN)");
+        return MOCO_ERR_INVALID;
+    }
+    if (workspace_bytes < bn_workspace_bytes()) { set_error("moco_bn_add_relu_bwd2: workspace too small"); return MOCO_ERR_WORKSPACE; }
+    cudaError_t e = launch_bn_add_relu_bwd(dy, dy2, x, residual, mask, M, C, *bn, shortcut, dx, dresidual, workspace,
+                                           static_cast<cudaStream_t>(stream_));
+    if (e == cudaErrorNotSupported) {
+        set_error("moco_bn_add_relu_bwd2: needs M >= 1 and C a power of two in [64, 2048] (M=%lld C=%d)", M, C);
         return MOCO_ERR_UNSUPPORTED;
     }
     if (e != cudaSuccess) return cuda_fail("batch-norm backward kernels", e);

@@ -117,7 +117,9 @@ cudaError_t launch_maxpool_fwd(const void* x, void* y, void* idx, int N, int H, 
                                const float* bn_mean = nullptr, const float* bn_invstd = nullptr,
                                const float* bn_gamma = nullptr, const float* bn_beta = nullptr,
                                const float* eval_scale = nullptr, const float* eval_shift = nullptr);
-cudaError_t launch_maxpool_bwd(const void* dy, const void* idx, void* dx, int N, int H, int W, int C, cudaStream_t stream);
+// dy2: nullable; a second gradient of the pooled output, added to dy (bf16 rounding of the sum) before the gather
+cudaError_t launch_maxpool_bwd(const void* dy, const void* dy2, const void* idx, void* dx, int N, int H, int W, int C,
+                               cudaStream_t stream);
 cudaError_t launch_crop_to_s2d(const void* src, int src_dtype, long long img_stride, __nv_bfloat16* dst, int N, int H, int W,
                                cudaStream_t stream, const int64_t* src_rows);
 size_t bn_workspace_bytes();
@@ -130,9 +132,10 @@ cudaError_t launch_bn_bwd(const void* dy, const void* x, const void* y, long lon
 using BnLayer = moco_bn_layer;
 cudaError_t launch_bn_add_relu_fwd(const void* x, const void* res, void* y, void* mask, long long M, int C,
                                    const BnLayer& bn, const BnLayer* sc, void* ws, cudaStream_t stream);
-cudaError_t launch_bn_add_relu_bwd(const void* dy, const void* x, const void* res, const void* mask, long long M, int C,
-                                   const BnLayer& bn, const BnLayer* sc, void* dx, void* dres, void* ws,
-                                   cudaStream_t stream);
+// dy2: nullable; a second gradient of y, added to dy (bf16 rounding of the sum) before the mask
+cudaError_t launch_bn_add_relu_bwd(const void* dy, const void* dy2, const void* x, const void* res, const void* mask,
+                                   long long M, int C, const BnLayer& bn, const BnLayer* sc, void* dx, void* dres,
+                                   void* ws, cudaStream_t stream);
 cudaError_t launch_bn_relu_maxpool_fwd(const void* x, void* y, void* taps, int N, int H, int W, int C, const BnLayer& bn,
                                        void* ws, cudaStream_t stream);
 cudaError_t launch_bn_eval_act(const void* x, const void* res, void* y, long long M, int C, const float* scale,

@@ -36,9 +36,10 @@ class _Basic(nn.Module):
 
     def forward(self, x, avgpool=False):
         y = self.bn1(self.conv1(x))
+        r = bn_mod.hand_over(x)                   # x's second consumer: its gradient is summed in x's producer
         if self.short is None:
-            return self.bn2(self.conv2(y), x, avgpool=avgpool)
-        return self.bn2(self.conv2(y), self.short[0](x), shortcut_bn=self.short[1], avgpool=avgpool)   # one BN group
+            return self.bn2(self.conv2(y), r, avgpool=avgpool)
+        return self.bn2(self.conv2(y), self.short[0](r), shortcut_bn=self.short[1], avgpool=avgpool)   # one BN group
 
 
 class _Bottleneck(nn.Module):
@@ -61,9 +62,10 @@ class _Bottleneck(nn.Module):
         """``avgpool``: return the global average pool of the output, [N, C] (the last block of the trunk)."""
         y = self.bn1(self.conv1(x))
         y = self.bn2(self.conv2(y))
+        r = bn_mod.hand_over(x)                   # x's second consumer: its gradient is summed in x's producer
         if self.short is None:
-            return self.bn3(self.conv3(y), x, avgpool=avgpool)
-        return self.bn3(self.conv3(y), self.short[0](x), shortcut_bn=self.short[1], avgpool=avgpool)   # one BN group
+            return self.bn3(self.conv3(y), r, avgpool=avgpool)
+        return self.bn3(self.conv3(y), self.short[0](r), shortcut_bn=self.short[1], avgpool=avgpool)   # one BN group
 
 
 class StemConv(nn.Conv2d):

@@ -118,6 +118,8 @@ def main():
     us = collections.defaultdict(float)
     launches = collections.defaultdict(int)
     names = collections.defaultdict(lambda: collections.defaultdict(float))
+    name_launches = collections.defaultdict(lambda: collections.defaultdict(int))
+    pools = []                                          # (start, name, device us) of every max-pool launch
     for ev in prof.events():
         t = ev.device_time
         if t <= 0:
@@ -126,6 +128,26 @@ def main():
         us[cls] += t
         launches[cls] += 1
         names[cls][ev.name] += t
+        name_launches[cls][ev.name] += 1
+        if cls == "maxpool":
+            pools.append((ev.time_range.start, ev.name, t))
+    # the stem's pool launches in step order (forward of each encoder, then the backward), with algorithmic GB/s:
+    # input [N, H/2, W/2, 64] bf16 after the stride-2 stem convolution, pooled to [N, H/4, W/4, 64] + 1 tap byte each
+    pools.sort()
+    per_step = len(pools) // args.steps if args.steps else 0
+    H = inputs.shape[-1] // 2
+    Ho = (H - 1) // 2 + 1
+    x_bytes, y_bytes = N * H * H * 64 * 2, N * Ho * Ho * 64 * 2
+    maxpool_launches = []
+    for i in range(per_step):
+        runs = pools[i::per_step]
+        name = runs[0][1]
+        mean_us = sum(r[2] for r in runs) / len(runs)
+        # forward: x, y + taps; backward: dy + taps (+ dy2, the kSum instance), dx
+        nbytes = (x_bytes + y_bytes * 3 // 2) if "fwd" in name else (y_bytes * 3 // 2 + x_bytes)
+        if "bwd_kernel<true>" in name:
+            nbytes += y_bytes
+        maxpool_launches.append({"kernel": name[:80], "us": mean_us, "bytes": nbytes, "GB_s": nbytes / mean_us / 1e3})
     total = sum(us.values())
     gpu, watts = card()
     line = {
@@ -140,6 +162,10 @@ def main():
         # the kernels behind the catch-all classes, so that a misfiled kernel is visible
         "top_kernels": {c: [[n[:120], t / 1e3 / args.steps] for n, t in sorted(names[c].items(), key=lambda kv: -kv[1])[:4]]
                         for c in ("other", "aten_other", "conv_other", "gemm") if c in names},
+        # every element-wise ATen kernel: [name, launches per step, ms per step]
+        "aten_elementwise_kernels": [[n[:160], name_launches["aten_elementwise"][n] / args.steps, t / 1e3 / args.steps]
+                                     for n, t in sorted(names["aten_elementwise"].items(), key=lambda kv: -kv[1])],
+        "maxpool_launches": maxpool_launches,
     }
     print(json.dumps(line))
 
