@@ -27,7 +27,7 @@
 extern "C" {
 #endif
 
-#define MOCO_B200_ABI_VERSION 3 /* 3: + moco_bn_*, moco_maxpool3x3s2_*, moco_crop_s2d_bf16 (additive) */
+#define MOCO_B200_ABI_VERSION 3 /* 3: + moco_bn_*, moco_maxpool3x3s2_*, moco_crop_s2d_bf16, moco_conv1x1_* (additive) */
 
 enum {
     MOCO_OK = 0,
@@ -335,6 +335,35 @@ int moco_bn_add_relu_bwd(const void* dy, const void* x, const void* residual, co
 int moco_bn_add_relu_bwd2(const void* dy, const void* dy2, const void* x, const void* residual, const void* mask,
                           long long M, int C, const moco_bn_layer* bn, const moco_bn_layer* shortcut_or_null, void* dx,
                           void* dresidual_or_null, void* workspace, size_t workspace_bytes, void* stream);
+
+/* The training forward of moco_bn_fwd_train / moco_bn_add_relu_fwd_train for BatchNorms whose batch statistics are
+ * already computed (moco_conv1x1_bn_stats): `stats_given` bit MOCO_BN_STATS_GIVEN says bn's save_mean / save_invstd
+ * (and its running statistics) are final, MOCO_BN_SC_STATS_GIVEN the same of the shortcut BN.  A layer whose bit is
+ * clear gets its statistics pass here, as in those calls; then one element-wise pass writes
+ *     y = relu?(bn(x) [+ r]),   r = residual, or bf16(shortcut_bn(residual)) with a shortcut BN (residual required),
+ * and the mask bits (nullable) as moco_bn_add_relu_fwd_train does.  Same apply kernel, so with the same statistics
+ * the outputs are bit-identical to those calls.  workspace may be NULL when no statistics pass runs.  One launch plus
+ * one per statistics pass. */
+enum { MOCO_BN_STATS_GIVEN = 1, MOCO_BN_SC_STATS_GIVEN = 2 };
+int moco_bn_fwd_train_given(const void* x, const void* residual_or_null, void* y, void* mask_or_null, long long M,
+                            int C, int relu, const moco_bn_layer* bn, const moco_bn_layer* shortcut_or_null,
+                            int stats_given, void* workspace, size_t workspace_bytes, void* stream);
+
+/* ------------------------------------------------------------------------
+ * 1x1 / stride 1 convolution forward with the following training BatchNorm's batch statistics: in NHWC the
+ * convolution is the GEMM  y[M, Cout] = x[M, Cin] . w[Cout, Cin]^T  (bf16 operands, fp32 accumulation, y rounded to
+ * bf16 once), and the statistics are those of y as rounded, finished as moco_bn_fwd_train's statistics pass does
+ * (mean and biased variance over the M rows, save_mean / save_invstd, running_mean / running_var with the unbiased
+ * variance, num_batches_tracked += 1).  Only bn's running_*, num_batches_tracked, momentum, eps and save_* are used.
+ * Follow it with moco_bn_fwd_train_given.  One launch on Hopper tensor cores (wgmma, TMA); deterministic.
+ *
+ * x: bf16 [M, Cin] (NHWC storage), w: bf16 [Cout, Cin] (the [Cout, Cin, 1, 1] weight), y: bf16 [M, Cout]; all
+ * 16-byte aligned.  Cin a multiple of 64 in [64, 65536], Cout a multiple of 64 in [64, 4096], M >= 1.
+ * workspace: >= moco_conv1x1_workspace_bytes() bytes, ZEROED ONCE before its first use, then private to one stream.
+ * ---------------------------------------------------------------------- */
+size_t moco_conv1x1_workspace_bytes(void);
+int moco_conv1x1_bn_stats(const void* x, const void* w, void* y, long long M, int Cin, int Cout,
+                          const moco_bn_layer* bn, void* workspace, size_t workspace_bytes, void* stream);
 
 /* The stem's BatchNorm + ReLU followed by its 3x3 / stride 2 / pad 1 max pooling, without writing the BatchNorm's
  * output: bit-identical to moco_bn_fwd_train (relu = 1, no residual) + moco_maxpool3x3s2_fwd.  The statistics pass,

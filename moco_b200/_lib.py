@@ -18,6 +18,7 @@ NCE_AUTO, NCE_FORCE_SIMT, NCE_CTA_PAIR, NCE_SINGLE_CTA = 0, 1, 2, 4
 NCE_TWO_PASS, NCE_ONE_PASS = 512, 1024
 ONE_PASS_MAX_INV_T = 25.0          # MOCO_ONE_PASS_MAX_INV_T (include/moco_b200.h)
 GATHER_AUTO, GATHER_LDG = 0, 1
+BN_STATS_GIVEN, BN_SC_STATS_GIVEN = 1, 2    # moco_bn_fwd_train_given `stats_given` bits
 
 
 
@@ -75,6 +76,11 @@ SIGNATURES = {
     "moco_bn_add_relu_bwd2": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int,
                                       POINTER(BnLayer), POINTER(BnLayer), c_void_p, c_void_p, c_void_p, c_size_t,
                                       c_void_p]),
+    "moco_bn_fwd_train_given": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, POINTER(BnLayer),
+                                        POINTER(BnLayer), c_int, c_void_p, c_size_t, c_void_p]),
+    "moco_conv1x1_workspace_bytes": (c_size_t, []),
+    "moco_conv1x1_bn_stats": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, POINTER(BnLayer), c_void_p,
+                                      c_size_t, c_void_p]),
     "moco_bn_relu_maxpool_fwd_train": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                                POINTER(BnLayer), c_void_p, c_size_t, c_void_p]),
     "moco_bn_eval_act": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_int, c_void_p,
@@ -136,7 +142,7 @@ class _Counting:
 
     _PER_CALL = {"moco_nce_shard_stats": 3, "moco_nce_shard_merge": 1, "moco_nce_shard_dq": 2,
                  "moco_nce_shard_dq_finish": 1, "moco_nce_shard_dq_finish_peers": 1, "moco_queue_enqueue_shard": 1, "moco_queue_enqueue": 1, "moco_f32_to_bf16": 1, "moco_shuffle_gather": 1, "moco_shuffle_gather_sync": 1, "moco_crop_gather_nhwc_bf16": 1,
-                 "moco_ema_update": 1, "moco_crop_to_nhwc_bf16": 1, "moco_bn_fwd_train": 2, "moco_bn_bwd": 2, "moco_bn_add_relu_bwd": 2, "moco_bn_add_relu_bwd2": 2, "moco_bn_relu_maxpool_fwd_train": 2, "moco_bn_eval_act": 1, "moco_bn_relu_maxpool_eval": 1, "moco_bn_eval_act_avgpool": 1, "moco_crop_s2d_bf16": 1, "moco_maxpool3x3s2_fwd": 1, "moco_maxpool3x3s2_bwd": 1, "moco_maxpool3x3s2_bwd2": 1,
+                 "moco_ema_update": 1, "moco_crop_to_nhwc_bf16": 1, "moco_bn_fwd_train": 2, "moco_bn_bwd": 2, "moco_bn_add_relu_bwd": 2, "moco_bn_add_relu_bwd2": 2, "moco_bn_relu_maxpool_fwd_train": 2, "moco_bn_eval_act": 1, "moco_bn_relu_maxpool_eval": 1, "moco_bn_eval_act_avgpool": 1, "moco_crop_s2d_bf16": 1, "moco_conv1x1_bn_stats": 1, "moco_maxpool3x3s2_fwd": 1, "moco_maxpool3x3s2_bwd": 1, "moco_maxpool3x3s2_bwd2": 1,
                  "moco_signal_barrier": 1, "moco_nce_bwd_dense": 1}
 
     def __init__(self, lib):
@@ -151,6 +157,9 @@ class _Counting:
                 setattr(self, name, self._wrap_flags(fn, 11))
             elif name == "moco_bn_add_relu_fwd_train":  # + the shortcut BN's statistics pass
                 setattr(self, name, self._wrap_count(fn, lambda a: 3 if a[7] is not None else 2))
+            elif name == "moco_bn_fwd_train_given":     # the apply pass + the statistics passes not given
+                setattr(self, name, self._wrap_count(fn, lambda a: 1 + (not a[9] & BN_STATS_GIVEN)
+                                                     + (a[8] is not None and not a[9] & BN_SC_STATS_GIVEN)))
             elif name in self._PER_CALL:
                 setattr(self, name, self._wrap(fn, self._PER_CALL[name]))
             else:

@@ -57,11 +57,14 @@ def set_fused(flag: bool) -> None:
     _enabled = bool(flag)
 
 
-def _workspace(device):
-    key = (device.index, torch.cuda.current_stream(device).cuda_stream)
+def _workspace(device, conv=False):
+    """The stream's workspace of the BatchNorm entry points, or (conv=True) of moco_conv1x1_bn_stats."""
+    key = (device.index, torch.cuda.current_stream(device).cuda_stream, conv)
     ws = _workspaces.get(key)
     if ws is None:
-        ws = torch.zeros(_lib.load().moco_bn_workspace_bytes(), dtype=torch.uint8, device=device)   # zeroed once
+        lib = _lib.load()
+        nbytes = lib.moco_conv1x1_workspace_bytes() if conv else lib.moco_bn_workspace_bytes()
+        ws = torch.zeros(nbytes, dtype=torch.uint8, device=device)   # zeroed once
         _workspaces[key] = ws
     return ws
 
@@ -91,24 +94,34 @@ class _BatchNormActFn(torch.autograd.Function):
     """y = relu?(batch_norm_train(x) [+ residual]); x, residual, y bf16 channels_last; weight / bias fp32."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, residual, running_mean, running_var, num_batches_tracked, momentum, eps, relu):
+    def forward(ctx, x, weight, bias, residual, running_mean, running_var, num_batches_tracked, momentum, eps, relu,
+                given=None):
+        """given: (mean, invstd) already computed by the producing convolution (:func:`conv1x1_stats`), which also
+        updated the running statistics: only the apply pass runs."""
         lib = _lib.load()
         N, C, H, W = x.shape
         M = N * H * W
         y = torch.empty_like(x)                                   # keeps the channels_last strides
-        mean = torch.empty(C, dtype=torch.float32, device=x.device)
-        invstd = torch.empty_like(mean)
-        ws = _workspace(x.device)
-        # algorithmic bytes: statistics read x; apply reads x (+ residual) and writes y
-        code = _timed("bn_fwd", M * C * 2 * (3 + (residual is not None)), lambda: lib.moco_bn_fwd_train(
-            x.data_ptr(), residual.data_ptr() if residual is not None else None, y.data_ptr(), M, C,
-            weight.data_ptr(), bias.data_ptr(),
-            running_mean.data_ptr() if running_mean is not None else None,
-            running_var.data_ptr() if running_var is not None else None,
-            num_batches_tracked.data_ptr() if num_batches_tracked is not None else None,
-            float(momentum), float(eps), int(relu), mean.data_ptr(), invstd.data_ptr(), ws.data_ptr(), ws.numel(),
-            _lib.cur_stream()))
-        _lib.check(code, "moco_bn_fwd_train")
+        ptr = lambda t: t.data_ptr() if t is not None else None
+        if given is not None:
+            mean, invstd = given
+            bn = _layer(weight, bias, mean, invstd, (running_mean, running_var, num_batches_tracked, momentum, eps))
+            # algorithmic bytes: apply reads x (+ residual) and writes y
+            code = _timed("bn_fwd", M * C * 2 * (2 + (residual is not None)), lambda: lib.moco_bn_fwd_train_given(
+                x.data_ptr(), ptr(residual), y.data_ptr(), None, M, C, int(relu), bn, None, _lib.BN_STATS_GIVEN,
+                None, 0, _lib.cur_stream()))
+            _lib.check(code, "moco_bn_fwd_train_given")
+        else:
+            mean = torch.empty(C, dtype=torch.float32, device=x.device)
+            invstd = torch.empty_like(mean)
+            ws = _workspace(x.device)
+            # algorithmic bytes: statistics read x; apply reads x (+ residual) and writes y
+            code = _timed("bn_fwd", M * C * 2 * (3 + (residual is not None)), lambda: lib.moco_bn_fwd_train(
+                x.data_ptr(), ptr(residual), y.data_ptr(), M, C, weight.data_ptr(), bias.data_ptr(),
+                ptr(running_mean), ptr(running_var), ptr(num_batches_tracked),
+                float(momentum), float(eps), int(relu), mean.data_ptr(), invstd.data_ptr(), ws.data_ptr(), ws.numel(),
+                _lib.cur_stream()))
+            _lib.check(code, "moco_bn_fwd_train")
         ctx.relu = bool(relu)
         ctx.has_res = residual is not None
         # the ReLU mask of the backward is recomputed from x unless a residual went into it
@@ -143,7 +156,7 @@ class _BatchNormActFn(torch.autograd.Function):
             int(ctx.has_res), dx.data_ptr(), dres_ptr, dgamma.data_ptr(), dbeta.data_ptr(),
             ws.data_ptr(), ws.numel(), _lib.cur_stream()))
         _lib.check(code, "moco_bn_bwd")
-        return dx, dgamma, dbeta, dres, None, None, None, None, None, None
+        return dx, dgamma, dbeta, dres, None, None, None, None, None, None, None
 
 
 def _layer(weight, bias, mean, invstd, stats=None, dgamma=None, dbeta=None):
@@ -161,26 +174,40 @@ class _BatchNormAddReluFn(torch.autograd.Function):
     materialised.  Same values as _BatchNormActFn (+ the shortcut BN's own pass)."""
 
     @staticmethod
-    def forward(ctx, x, residual, weight, bias, sc_weight, sc_bias, stats, sc_stats, want_mask):
+    def forward(ctx, x, residual, weight, bias, sc_weight, sc_bias, stats, sc_stats, want_mask, given=None,
+                sc_given=None):
+        """given / sc_given: (mean, invstd) of the BatchNorm / the shortcut BN already computed by the producing
+        convolution (:func:`conv1x1_stats`), which also updated its running statistics; that statistics pass is
+        skipped."""
         lib = _lib.load()
         N, C, H, W = x.shape
         M = N * H * W
         y = torch.empty_like(x)
         mask = torch.empty((M, C // 8), dtype=torch.uint8, device=x.device) if want_mask else None
         f32 = lambda: torch.empty(C, dtype=torch.float32, device=x.device)
-        mean, invstd = f32(), f32()
+        mean, invstd = given if given is not None else (f32(), f32())
         bn = _layer(weight, bias, mean, invstd, stats)
         sc, sc_mean, sc_invstd = None, None, None
         if sc_weight is not None:
-            sc_mean, sc_invstd = f32(), f32()
+            sc_mean, sc_invstd = sc_given if sc_given is not None else (f32(), f32())
             sc = _layer(sc_weight, sc_bias, sc_mean, sc_invstd, sc_stats)
         ws = _workspace(x.device)
-        # algorithmic bytes: statistics read x (+ the shortcut input); apply reads x and residual, writes y (+ mask bits)
-        nbytes = M * C * 2 * (4 + (sc is not None)) + (M * C // 8 if want_mask else 0)
-        code = _timed("bn_fwd", nbytes, lambda: lib.moco_bn_add_relu_fwd_train(
-            x.data_ptr(), residual.data_ptr(), y.data_ptr(), mask.data_ptr() if mask is not None else None, M, C, bn, sc,
-            ws.data_ptr(), ws.numel(), _lib.cur_stream()))
-        _lib.check(code, "moco_bn_add_relu_fwd_train")
+        flags = (_lib.BN_STATS_GIVEN if given is not None else 0) | (_lib.BN_SC_STATS_GIVEN if sc_given is not None else 0)
+        # algorithmic bytes: statistics read x (+ the shortcut input) unless given; apply reads x and residual, writes
+        # y (+ mask bits)
+        passes = (given is None) + (sc is not None and sc_given is None)
+        nbytes = M * C * 2 * (3 + passes) + (M * C // 8 if want_mask else 0)
+        mask_ptr = mask.data_ptr() if mask is not None else None
+        if flags:
+            code = _timed("bn_fwd", nbytes, lambda: lib.moco_bn_fwd_train_given(
+                x.data_ptr(), residual.data_ptr(), y.data_ptr(), mask_ptr, M, C, 1, bn, sc, flags, ws.data_ptr(),
+                ws.numel(), _lib.cur_stream()))
+            _lib.check(code, "moco_bn_fwd_train_given")
+        else:
+            code = _timed("bn_fwd", nbytes, lambda: lib.moco_bn_add_relu_fwd_train(
+                x.data_ptr(), residual.data_ptr(), y.data_ptr(), mask_ptr, M, C, bn, sc, ws.data_ptr(), ws.numel(),
+                _lib.cur_stream()))
+            _lib.check(code, "moco_bn_add_relu_fwd_train")
         ctx.save_for_backward(x, residual if sc is not None else None, mask, weight, mean, invstd, sc_weight, sc_mean,
                               sc_invstd)
         return y
@@ -222,7 +249,7 @@ class _BatchNormAddReluFn(torch.autograd.Function):
                 dy.data_ptr(), dy2.data_ptr(), x.data_ptr(), ptr(residual), mask.data_ptr(), M, C, bn, sc,
                 dx.data_ptr(), ptr(dres), ws.data_ptr(), ws.numel(), _lib.cur_stream()))
             _lib.check(code, "moco_bn_add_relu_bwd2")
-        return dx, dres, dgamma, dbeta, sc_dgamma, sc_dbeta, None, None, None
+        return dx, dres, dgamma, dbeta, sc_dgamma, sc_dbeta, None, None, None, None, None
 
 
 class _BatchNormReluMaxPoolFn(torch.autograd.Function):
@@ -309,6 +336,89 @@ def hand_over(x):
     return _HandOverFn.apply(x, node)
 
 
+class _Conv1x1StatsFn(torch.autograd.Function):
+    """y = conv2d(x, w) of a 1x1 / stride 1 convolution without bias (x bf16 channels_last, w the bf16 weight
+    [Cout, Cin, 1, 1]) and the batch statistics of the training BatchNorm that reads y: one launch of
+    ``moco_conv1x1_bn_stats``, which also updates that BatchNorm's running statistics.  Returns (y, mean, invstd).
+    The backward is the convolution's own, ``aten.convolution_backward`` with the arguments autograd gives it for
+    ``F.conv2d``, so the gradients of a given forward are unchanged."""
+
+    @staticmethod
+    def forward(ctx, x, w, stats):
+        lib = _lib.load()
+        N, Cin, H, W = x.shape
+        Cout = w.shape[0]
+        y = torch.empty((N, Cout, H, W), dtype=torch.bfloat16, device=x.device, memory_format=torch.channels_last)
+        mean = torch.empty(Cout, dtype=torch.float32, device=x.device)
+        invstd = torch.empty_like(mean)
+        ws = _workspace(x.device, conv=True)
+        _lib.check(lib.moco_conv1x1_bn_stats(x.data_ptr(), w.data_ptr(), y.data_ptr(), N * H * W, Cin, Cout,
+                                             _layer(None, None, mean, invstd, stats), ws.data_ptr(), ws.numel(),
+                                             _lib.cur_stream()), "moco_conv1x1_bn_stats")
+        ctx.save_for_backward(x, w)
+        ctx.mark_non_differentiable(mean, invstd)
+        return y, mean, invstd
+
+    @staticmethod
+    def backward(ctx, dy, _dmean, _dinvstd):
+        x, w = ctx.saved_tensors
+        dx, dw, _ = torch.ops.aten.convolution_backward(
+            dy, x, w, None, [1, 1], [0, 0], [1, 1], False, [0, 0], 1,
+            [ctx.needs_input_grad[0], ctx.needs_input_grad[1], False])
+        return dx, dw, None
+
+
+# (Cin, Cout) of ResNet-50's stride-1 1x1 convolutions on which moco_conv1x1_bn_stats + the apply pass measured more
+# than 3 % faster than cuDNN's convolution + the statistics and apply passes at batch 256, on an H100 SXM at a 700 W
+# power limit (tools/conv1x1_times.py, results/conv1x1_times_h100.json): 1.08-1.23x on stages 1-2 and on the 256 -> 1024
+# conv3 of stage 3.  The K-heavy ones of stages 3-4 (1024 -> 256, 1024 -> 512, 2048 -> 512, 512 -> 2048) measured
+# 0.73-0.97x and keep cuDNN.
+_CONV1X1_WINS = frozenset({(64, 64), (256, 64), (64, 256), (256, 128), (512, 128), (128, 512), (512, 256),
+                           (256, 1024)})
+
+
+def _conv1x1_wins(M, Cin, Cout):
+    """The shapes moco_conv1x1_bn_stats was measured to win on (_CONV1X1_WINS) at batch 256's row counts; smaller
+    batches were not measured and keep cuDNN."""
+    return M >= 50176 and (Cin, Cout) in _CONV1X1_WINS
+
+
+def _conv1x1_ok(conv, bn, x, residual=None, shortcut_bn=None):
+    """conv(x) may run as moco_conv1x1_bn_stats: a 1x1 / stride 1 convolution without bias, groups, dilation or
+    padding computing in bf16 on bf16 channels_last activations, channels multiples of 64, and bn (with ``residual``,
+    and ``shortcut_bn`` on ``residual`` when bn is a downsample block's bn3) taking its training kernels on the
+    output."""
+    w = conv.weight
+    if not (_enabled and isinstance(conv, nn.Conv2d) and type(conv).forward is nn.Conv2d.forward
+            and conv.kernel_size == (1, 1) and conv.stride == (1, 1) and conv.padding == (0, 0)
+            and conv.dilation == (1, 1) and conv.groups == 1 and conv.bias is None and _rows_ok(x)
+            and w.is_cuda and w.device == x.device and x.shape[1] == w.shape[1]):
+        return False
+    if not (w.dtype == torch.bfloat16 or (torch.is_autocast_enabled("cuda")
+                                         and torch.get_autocast_dtype("cuda") == torch.bfloat16)):
+        return False
+    N, Cin, H, W = x.shape
+    Cout = w.shape[0]
+    out = torch.Size((N, Cout, H, W))
+    if Cin % 64 != 0 or Cout % 64 != 0 or not bn._fusable_shape(out, residual):
+        return False
+    if shortcut_bn is not None and not (bn.relu and not shortcut_bn.relu and shortcut_bn._fusable(residual, None)):
+        return False
+    return _conv1x1_wins(N * H * W, Cin, Cout)
+
+
+def conv1x1_stats(conv, bn, x, residual=None, shortcut_bn=None):
+    """(conv(x), stats): stats = the batch statistics of the training BatchNorm ``bn`` on conv(x), computed with the
+    convolution by moco_conv1x1_bn_stats (``bn``'s running statistics are updated), to be passed to ``bn(...,
+    stats=stats)``; None where that kernel does not take the convolution (see :func:`_conv1x1_ok`), which then runs
+    as ``conv(x)``.  ``residual`` / ``shortcut_bn``: what ``bn`` will be called with."""
+    if not _conv1x1_ok(conv, bn, x, residual, shortcut_bn):
+        return conv(x), None
+    w = conv.weight.to(torch.bfloat16).contiguous()     # outside the Function: its autograd gives the fp32 gradient
+    y, mean, invstd = _Conv1x1StatsFn.apply(x, w, bn._stats())
+    return y, (mean, invstd)
+
+
 class BatchNormAct2d(nn.BatchNorm2d):
     """``nn.BatchNorm2d`` + optional residual add + optional ReLU (``forward(x, residual=None)``)."""
 
@@ -320,11 +430,15 @@ class BatchNormAct2d(nn.BatchNorm2d):
         self._fold = None
 
     def _fusable(self, x, residual):
+        return _rows_ok(x) and self._fusable_shape(x.shape, residual)
+
+    def _fusable_shape(self, shape, residual):
+        """The training kernels take a bf16 channels_last input of this shape (and this residual)."""
         C = self.num_features
         return (_enabled and self.training and self.affine and self.momentum is not None
-                and _rows_ok(x) and (residual is None or _rows_ok(residual, x))
-                and 64 <= C <= 2048 and (C & (C - 1)) == 0 and x.shape[1] == C
-                and x.numel() // C > 1                 # a single value per channel: nn.BatchNorm2d's own error
+                and (residual is None or (_rows_ok(residual) and residual.shape == shape))
+                and 64 <= C <= 2048 and (C & (C - 1)) == 0 and shape[1] == C
+                and shape.numel() // C > 1             # a single value per channel: nn.BatchNorm2d's own error
                 and self.weight.dtype == torch.float32 and self.weight.is_cuda
                 and (self.running_mean is None or self.running_mean.dtype == torch.float32))
 
@@ -379,30 +493,36 @@ class BatchNormAct2d(nn.BatchNorm2d):
         return (self.running_mean, self.running_var, self.num_batches_tracked if self.track_running_stats else None,
                 self.momentum, self.eps)
 
-    def forward(self, x, residual=None, shortcut_bn=None, avgpool=False):
+    def forward(self, x, residual=None, shortcut_bn=None, avgpool=False, stats=None, sc_stats=None):
         """``shortcut_bn``: a downsample block's shortcut BatchNorm (no ReLU); ``residual`` is then its input, the
         shortcut convolution's raw output, and ``y = relu?(bn(x) + shortcut_bn(residual))``.  ``avgpool``: return
-        the global average pool of y, flattened to [N, C] (fp32 from the frozen path, y's dtype otherwise)."""
+        the global average pool of y, flattened to [N, C] (fp32 from the frozen path, y's dtype otherwise).
+        ``stats`` / ``sc_stats``: the batch statistics of x / of the shortcut input from :func:`conv1x1_stats`, which
+        only gives them where the training kernels take this call."""
         if avgpool:
             if (shortcut_bn is None or not shortcut_bn.relu and shortcut_bn._eval_ok(residual, None)) \
-                    and self._eval_ok(x, residual):
+                    and self._eval_ok(x, residual) and stats is None and sc_stats is None:
                 return self._eval(x, residual, shortcut_bn, True)
-            return torch.flatten(F.adaptive_avg_pool2d(self.forward(x, residual, shortcut_bn), 1), 1)
+            return torch.flatten(F.adaptive_avg_pool2d(self.forward(x, residual, shortcut_bn, stats=stats,
+                                                                    sc_stats=sc_stats), 1), 1)
         if shortcut_bn is not None:
-            if not shortcut_bn.relu and self._eval_ok(x, residual) and shortcut_bn._eval_ok(residual, None):
+            if (not shortcut_bn.relu and self._eval_ok(x, residual) and shortcut_bn._eval_ok(residual, None)
+                    and stats is None and sc_stats is None):
                 return self._eval(x, residual, shortcut_bn, False)
             if (self.relu and not shortcut_bn.relu and self._fusable(x, residual)
                     and shortcut_bn._fusable(residual, None)):
-                return self._add_relu(x, residual, shortcut_bn)
-            residual = shortcut_bn(residual)
-        if self._eval_ok(x, residual):
+                return self._add_relu(x, residual, shortcut_bn, stats, sc_stats)
+            residual = shortcut_bn(residual, stats=sc_stats)
+        if self._eval_ok(x, residual) and stats is None:
             return self._eval(x, residual, None, False)
         if self._fusable(x, residual):
             if self.relu and residual is not None:
-                return self._add_relu(x, residual, None)
+                return self._add_relu(x, residual, None, stats)
             return _BatchNormActFn.apply(x, self.weight, self.bias, residual, self.running_mean, self.running_var,
                                          self.num_batches_tracked if self.track_running_stats else None,
-                                         self.momentum, self.eps, self.relu)
+                                         self.momentum, self.eps, self.relu, stats)
+        if stats is not None:
+            raise RuntimeError("moco_b200: batch statistics given to a BatchNorm that cannot take them")
         y = super().forward(x)
         if residual is not None:
             y = y + residual
@@ -426,12 +546,13 @@ class BatchNormAct2d(nn.BatchNorm2d):
             return _BatchNormReluMaxPoolFn.apply(x, self.weight, self.bias, self._stats())
         return pool(self(x))
 
-    def _add_relu(self, x, residual, sc):
+    def _add_relu(self, x, residual, sc, stats=None, sc_stats=None):
         params = (x, residual, self.weight, self.bias) + ((sc.weight, sc.bias) if sc is not None else ())
         want_mask = torch.is_grad_enabled() and any(t.requires_grad for t in params)
         return _BatchNormAddReluFn.apply(x, residual, self.weight, self.bias,
                                          sc.weight if sc is not None else None, sc.bias if sc is not None else None,
-                                         self._stats(), sc._stats() if sc is not None else None, want_mask)
+                                         self._stats(), sc._stats() if sc is not None else None, want_mask,
+                                         stats, sc_stats)
 
     def extra_repr(self):
         return super().extra_repr() + f", relu={self.relu}"

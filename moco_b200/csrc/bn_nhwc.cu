@@ -27,21 +27,17 @@
 // that the variance does not cancel.
 // Element-wise passes: thread t keeps the coefficients of its 8 channels in registers (its channel group never
 // changes because the grid stride is a multiple of the row length in vectors) and streams 16-byte vectors linearly.
+#include "bn_reduce.cuh"
 #include "common.cuh"
 
 #include <cuda_bf16.h>
 
 namespace moco {
 
-constexpr int kBnThreads = 256;
-constexpr int kBnSlab = 64;                          // channels per reduction CTA
-constexpr int kBnLanes = kBnSlab / 8;                // 16-byte vectors per slab row
-constexpr int kBnRows = kBnThreads / kBnLanes;       // rows per pass
 constexpr int kBnMaxSlabs = 32;                      // C <= 2048
 constexpr int kBnMaxPartial = 3 * kBnSlab;           // floats per CTA partial: up to three sums per channel
 // (16-byte loads in flight per thread and operand, resident CTAs per SM) of each kernel; every grid is one resident
 // wave (tools/bn_kernel_times.py times the variants over the layers of ResNet-50).
-constexpr int kBnStatsUnroll = 8, kBnStatsCtas = 2;
 constexpr int kBnApplyUnroll = 8, kBnApplyCtas = 2;
 constexpr int kBnBwdReduceUnroll = 4, kBnBwdReduceCtas = 2;
 constexpr int kBnBwdApplyUnroll = 2, kBnBwdApplyCtas = 3;
@@ -50,97 +46,12 @@ constexpr int kBnBwdApplySumUnroll = 2, kBnBwdApplySumCtas = 2; // with a second
 constexpr int kBnSms = 132;
 constexpr int kBnMaxCtas = kBnSms * 4;               // workspace sizing: no reduction grid is larger
 
-__device__ __forceinline__ void unpack8(const uint4& u, float* f) {
-    const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        const float2 t = __bfloat1622float2(h[k]);
-        f[2 * k] = t.x;
-        f[2 * k + 1] = t.y;
-    }
-}
-
 __device__ __forceinline__ uint4 pack8(const float* f) {
     uint4 u;
     __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&u);
 #pragma unroll
     for (int k = 0; k < 4; ++k) h[k] = __floats2bfloat162_rn(f[2 * k], f[2 * k + 1]);
     return u;
-}
-
-// Sum the 8 * S per-thread accumulators (S per-channel sums of 8 channels) over the CTA's 32 row groups.  Returns, in
-// threads j < 64 * S, element j of the CTA partial: j = v * 8S + k with v = 16-byte lane (8 channels), k < 8 the first
-// sum, 8 <= k < 16 the second, 16 <= k < 24 the third.  Each element is added in the same order whatever S is.
-template <int S>
-__device__ __forceinline__ float slab_reduce(float (&acc)[8 * S], float* red /*[8 * 64S]*/) {
-    constexpr int P = S * kBnSlab;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < 8 * S; ++k) {
-        acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], 8);
-        acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], 16);
-    }
-    if (lane < 8) {
-#pragma unroll
-        for (int k = 0; k < 8 * S; ++k) red[warp * P + lane * 8 * S + k] = acc[k];
-    }
-    __syncthreads();
-    float t = 0.f;
-    if (threadIdx.x < P) {
-#pragma unroll
-        for (int w = 0; w < kBnThreads / 32; ++w) t += red[w * P + threadIdx.x];
-    }
-    return t;
-}
-
-// Publishes this CTA's partial (64S floats), and in the last CTA of the slab to arrive returns true with the slab
-// totals in tot[64S] (same element order as slab_reduce).  The R partials are added in a fixed order: warp w takes
-// partials w, w + 8, ... (lane l owns floats 4l .. 4l+3 of each 128-float chunk, one coalesced 512-byte read per
-// partial and chunk, 16 reads in flight), then the 8 warps' sums are added in warp order.
-template <int S>
-__device__ __forceinline__ bool slab_finish(float part, float* partial, unsigned int* counter, int slab, int r, int R,
-                                            double* tot /*[8 * 64S] shared*/, int* flag /*shared*/) {
-    constexpr int P = S * kBnSlab;
-    float* mine = partial + ((size_t)slab * R + r) * P;
-    if (threadIdx.x < P) mine[threadIdx.x] = part;
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        const unsigned int ticket = atomicAdd(counter, 1u);
-        *flag = (ticket == (unsigned int)(R - 1));
-    }
-    __syncthreads();
-    if (!*flag) return false;
-    __threadfence();
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const float4* base = reinterpret_cast<const float4*>(partial + (size_t)slab * R * P);
-    for (int c4 = lane; c4 < P / 4; c4 += 32) {
-        double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;
-        constexpr int kBatch = 16;
-        for (int q0 = warp; q0 < R; q0 += 8 * kBatch) {
-            float4 v[kBatch];
-#pragma unroll
-            for (int t = 0; t < kBatch; ++t) {
-                const int q = q0 + 8 * t;
-                v[t] = (q < R) ? __ldcg(base + (size_t)q * (P / 4) + c4) : make_float4(0.f, 0.f, 0.f, 0.f);
-            }
-#pragma unroll
-            for (int t = 0; t < kBatch; ++t) { s0 += v[t].x; s1 += v[t].y; s2 += v[t].z; s3 += v[t].w; }
-        }
-        double* mine_tot = tot + warp * P + c4 * 4;
-        mine_tot[0] = s0; mine_tot[1] = s1; mine_tot[2] = s2; mine_tot[3] = s3;
-    }
-    __syncthreads();
-    if (threadIdx.x < P) {
-        double t = 0.0;
-#pragma unroll
-        for (int w = 0; w < 8; ++w) t += tot[w * P + threadIdx.x];
-        __syncwarp();
-        tot[threadIdx.x] = t;                        // only this thread reads slot threadIdx.x (w = 0 above)
-    }
-    if (threadIdx.x == 0) *counter = 0u;             // re-armed for the next launch on this stream
-    __syncthreads();
-    return true;
 }
 
 struct BnStatsArgs {
@@ -204,22 +115,9 @@ bn_stats_kernel(const BnStatsArgs a) {
     const float part = slab_reduce<2>(acc, red);
     if (!slab_finish<2>(part, a.partial, a.counters + slab, slab, r, a.R, tot, &flag)) return;
     if (threadIdx.x < kBnSlab) {
-        const int c8 = threadIdx.x >> 3, k = threadIdx.x & 7;
         const int c = slab * kBnSlab + threadIdx.x;
-        const double s1 = tot[c8 * 16 + k], s2 = tot[c8 * 16 + 8 + k];
-        const double inv_m = 1.0 / (double)a.M;
-        const double md = s1 * inv_m;
-        double var = s2 * inv_m - md * md;
-        if (var < 0.0) var = 0.0;
-        const float shift = __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(a.x)[c]);
-        const float mean = (float)((double)shift + md);
-        a.mean[c] = mean;
-        a.invstd[c] = (float)(1.0 / sqrt(var + (double)a.eps));
-        if (a.running_mean != nullptr) {
-            const double unbiased = a.M > 1 ? var * ((double)a.M / (double)(a.M - 1)) : var;
-            a.running_mean[c] = (1.f - a.momentum) * a.running_mean[c] + a.momentum * mean;
-            a.running_var[c] = (1.f - a.momentum) * a.running_var[c] + a.momentum * (float)unbiased;
-        }
+        bn_stats_channel(tot, threadIdx.x, __bfloat162float(reinterpret_cast<const __nv_bfloat16*>(a.x)[c]), a.M, a.eps,
+                         a.momentum, c, a.mean, a.invstd, a.running_mean, a.running_var);
     }
     if (slab == 0 && threadIdx.x == 0 && a.num_batches_tracked != nullptr) *a.num_batches_tracked += 1;
 }
@@ -691,6 +589,10 @@ static void bn_reduce_plan(long long M, int C, int unroll, int ctas_per_sm, long
     *passes = np; *ppc = per; *R = (int)r;
 }
 
+void bn_stats_plan(long long M, int C, long long* passes, long long* ppc, int* R) {
+    bn_reduce_plan(M, C, kBnStatsUnroll, kBnStatsCtas, passes, ppc, R);
+}
+
 static int bn_apply_grid(long long V, int unroll, int ctas_per_sm) {
     long long g = (V + (long long)kBnThreads * unroll - 1) / ((long long)kBnThreads * unroll);
     if (g > kBnSms * ctas_per_sm) g = kBnSms * ctas_per_sm;
@@ -771,23 +673,30 @@ cudaError_t launch_bn_bwd(const void* dy, const void* x, const void* y, long lon
     return run_bwd_apply<kBnBwdApplyUnroll, kBnBwdApplyCtas, false>(p, stream);
 }
 
-cudaError_t launch_bn_add_relu_fwd(const void* x, const void* res, void* y, void* mask, long long M, int C,
-                                   const BnLayer& bn, const BnLayer* sc, void* ws, cudaStream_t stream) {
+cudaError_t launch_bn_fwd_given(const void* x, const void* res, void* y, void* mask, long long M, int C, int relu,
+                                const BnLayer& bn, const BnLayer* sc, int given, void* ws, cudaStream_t stream) {
     if (!bn_shape_ok(M, C)) return cudaErrorNotSupported;
-    cudaError_t e = stats_pass(x, M, C, bn.running_mean, bn.running_var, bn.num_batches_tracked, bn.momentum, bn.eps,
-                               bn.save_mean, bn.save_invstd, ws, stream);
-    if (e == cudaSuccess && sc != nullptr)
+    cudaError_t e = cudaSuccess;
+    if (!(given & MOCO_BN_STATS_GIVEN))
+        e = stats_pass(x, M, C, bn.running_mean, bn.running_var, bn.num_batches_tracked, bn.momentum, bn.eps,
+                       bn.save_mean, bn.save_invstd, ws, stream);
+    if (e == cudaSuccess && sc != nullptr && !(given & MOCO_BN_SC_STATS_GIVEN))
         e = stats_pass(res, M, C, sc->running_mean, sc->running_var, sc->num_batches_tracked, sc->momentum, sc->eps,
                        sc->save_mean, sc->save_invstd, ws, stream);
     if (e != cudaSuccess) return e;
     BnApplyArgs p{};
     p.x = static_cast<const uint4*>(x); p.res = static_cast<const uint4*>(res); p.y = static_cast<uint4*>(y);
     p.mask = static_cast<uint8_t*>(mask);
-    p.V = M * (C >> 3); p.C = C; p.relu = 1;
+    p.V = M * (C >> 3); p.C = C; p.relu = relu;
     p.mean = bn.save_mean; p.invstd = bn.save_invstd; p.gamma = bn.gamma; p.beta = bn.beta;
     if (sc == nullptr) return run_apply<kBnApplyUnroll, kBnApplyCtas, false>(p, stream);
     p.mean2 = sc->save_mean; p.invstd2 = sc->save_invstd; p.gamma2 = sc->gamma; p.beta2 = sc->beta;
     return run_apply<kBnApplyUnroll, kBnApplyCtas, true>(p, stream);
+}
+
+cudaError_t launch_bn_add_relu_fwd(const void* x, const void* res, void* y, void* mask, long long M, int C,
+                                   const BnLayer& bn, const BnLayer* sc, void* ws, cudaStream_t stream) {
+    return launch_bn_fwd_given(x, res, y, mask, M, C, 1, bn, sc, 0, ws, stream);
 }
 
 template <bool SUM>

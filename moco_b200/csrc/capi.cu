@@ -612,6 +612,60 @@ int moco_bn_add_relu_fwd_train(const void* x, const void* residual, void* y, voi
     return MOCO_OK;
 }
 
+int moco_bn_fwd_train_given(const void* x, const void* residual, void* y, void* mask, long long M, int C, int relu,
+                            const moco_bn_layer* bn, const moco_bn_layer* shortcut, int stats_given, void* workspace,
+                            size_t workspace_bytes, void* stream_) {
+    g_err[0] = 0;
+    const bool passes = !(stats_given & MOCO_BN_STATS_GIVEN) || (shortcut && !(stats_given & MOCO_BN_SC_STATS_GIVEN));
+    if (!x || !y || !bn_layer_fwd_ok(bn) || (shortcut && (!bn_layer_fwd_ok(shortcut) || !residual)) ||
+        (stats_given & ~(MOCO_BN_STATS_GIVEN | MOCO_BN_SC_STATS_GIVEN)) || (passes && !workspace) || misaligned16(x) ||
+        misaligned16(residual) || misaligned16(y) || misaligned16(workspace) || x == y || residual == y) {
+        set_error("moco_bn_fwd_train_given: bad argument (null / misaligned pointer, in-place, eps <= 0, one of "
+                  "running_mean / running_var, unknown stats_given bits; a shortcut BN needs residual, a statistics "
+                  "pass the workspace)");
+        return MOCO_ERR_INVALID;
+    }
+    if (passes && workspace_bytes < bn_workspace_bytes()) {
+        set_error("moco_bn_fwd_train_given: workspace too small");
+        return MOCO_ERR_WORKSPACE;
+    }
+    cudaError_t e = launch_bn_fwd_given(x, residual, y, mask, M, C, relu, *bn, shortcut, stats_given, workspace,
+                                        static_cast<cudaStream_t>(stream_));
+    if (e == cudaErrorNotSupported) {
+        set_error("moco_bn_fwd_train_given: needs M >= 1 and C a power of two in [64, 2048] (M=%lld C=%d)", M, C);
+        return MOCO_ERR_UNSUPPORTED;
+    }
+    if (e != cudaSuccess) return cuda_fail("batch-norm forward kernels", e);
+    return MOCO_OK;
+}
+
+size_t moco_conv1x1_workspace_bytes(void) { return conv1x1_workspace_bytes(); }
+
+int moco_conv1x1_bn_stats(const void* x, const void* w, void* y, long long M, int Cin, int Cout,
+                          const moco_bn_layer* bn, void* workspace, size_t workspace_bytes, void* stream_) {
+    g_err[0] = 0;
+    if (!x || !w || !y || !workspace || !bn || !bn->save_mean || !bn->save_invstd ||
+        (bn->running_mean == nullptr) != (bn->running_var == nullptr) || !(bn->eps > 0.f) || misaligned16(x) ||
+        misaligned16(w) || misaligned16(y) || misaligned16(workspace) || x == y || w == y) {
+        set_error("moco_conv1x1_bn_stats: bad argument (null / misaligned pointer, in-place, eps <= 0, one of "
+                  "running_mean / running_var)");
+        return MOCO_ERR_INVALID;
+    }
+    if (M < 1 || M > 0x7fffff80LL || Cin < 64 || Cin % 64 != 0 || Cin > 65536 || Cout < 64 || Cout % 64 != 0 ||
+        Cout > 4096) {
+        set_error("moco_conv1x1_bn_stats: needs 1 <= M < 2^31 - 128, Cin a multiple of 64 in [64, 65536] and Cout a "
+                  "multiple of 64 in [64, 4096] (M=%lld Cin=%d Cout=%d)", M, Cin, Cout);
+        return MOCO_ERR_UNSUPPORTED;
+    }
+    if (workspace_bytes < conv1x1_workspace_bytes()) {
+        set_error("moco_conv1x1_bn_stats: workspace too small");
+        return MOCO_ERR_WORKSPACE;
+    }
+    cudaError_t e = launch_conv1x1_bn_stats(x, w, y, M, Cin, Cout, *bn, workspace, static_cast<cudaStream_t>(stream_));
+    if (e != cudaSuccess) return cuda_fail("moco_conv1x1_bn_stats", e);
+    return MOCO_OK;
+}
+
 int moco_bn_add_relu_bwd(const void* dy, const void* x, const void* residual, const void* mask, long long M, int C,
                          const moco_bn_layer* bn, const moco_bn_layer* shortcut, void* dx, void* dresidual,
                          void* workspace, size_t workspace_bytes, void* stream_) {

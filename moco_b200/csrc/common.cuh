@@ -132,6 +132,9 @@ cudaError_t launch_bn_bwd(const void* dy, const void* x, const void* y, long lon
 using BnLayer = moco_bn_layer;
 cudaError_t launch_bn_add_relu_fwd(const void* x, const void* res, void* y, void* mask, long long M, int C,
                                    const BnLayer& bn, const BnLayer* sc, void* ws, cudaStream_t stream);
+// given: MOCO_BN_STATS_GIVEN / MOCO_BN_SC_STATS_GIVEN, the layers whose save_mean / save_invstd are already final
+cudaError_t launch_bn_fwd_given(const void* x, const void* res, void* y, void* mask, long long M, int C, int relu,
+                                const BnLayer& bn, const BnLayer* sc, int given, void* ws, cudaStream_t stream);
 // dy2: nullable; a second gradient of y, added to dy (bf16 rounding of the sum) before the mask
 cudaError_t launch_bn_add_relu_bwd(const void* dy, const void* dy2, const void* x, const void* res, const void* mask,
                                    long long M, int C, const BnLayer& bn, const BnLayer* sc, void* dx, void* dres,
@@ -146,6 +149,11 @@ cudaError_t launch_bn_eval_act_avgpool(const void* x, const void* res, float* fe
                                        const float* sc_shift, cudaStream_t stream);
 cudaError_t launch_bn_relu_maxpool_eval(const void* x, void* y, int N, int H, int W, int C, const float* scale,
                                         const float* shift, cudaStream_t stream);
+// rows of the statistics pass: passes of kBnRows rows, ppc passes per CTA (a multiple of kBnStatsUnroll), R CTAs
+void bn_stats_plan(long long M, int C, long long* passes, long long* ppc, int* R);
+size_t conv1x1_workspace_bytes();
+cudaError_t launch_conv1x1_bn_stats(const void* x, const void* w, void* y, long long M, int Cin, int Cout,
+                                    const BnLayer& bn, void* ws, cudaStream_t stream);
 int ema_chunk_elems();
 cudaError_t launch_ema(const void* segs, const int* chunk_prefix, int n_segs, int n_chunks, float m,
                        float one_minus_m, cudaStream_t stream);

@@ -1,0 +1,287 @@
+// 1x1 convolution forward on Hopper tensor cores (sm_90a) with the batch statistics of the following BatchNorm taken
+// in the epilogue: the bottleneck blocks' conv1 -> bn1, conv3 -> bn3 and stride-1 shortcut -> BatchNorm
+// (moco/models/resnet.py:74-102,139-143).  In NHWC a 1x1 / stride 1 convolution is the GEMM
+//     y[M, Cout] = x[M, Cin] . w[Cout, Cin]^T           (M = N*H*W; x, w, y bf16, fp32 accumulation, y rounded once)
+// and the statistics are those of y AS ROUNDED to bf16, the tensor the BatchNorm reads.  They replace that BatchNorm's
+// statistics pass (bn_nhwc.cu: bn_stats_kernel), which would read y back from HBM once more.
+//
+// Layout of the work.  384 threads: warps 0-3 and 4-7 are two consumer warpgroups, each owning 64 rows of the CTA's
+// 128-row tile; one thread of warp 8 is the TMA producer (setmaxnreg: 40 / 232 registers per thread).  A CTA owns one
+// BN-column slice of y (BN = 128, or 64 when Cout is not a multiple of 128) and a contiguous range of 128-row tiles.
+// Per tile and 64-wide K chunk the producer loads the x slab [128 x 64] and the w slab [BN x 64] into a ring of smem
+// stages; each warpgroup runs wgmma m64nBNk16 x 4 from smem (both K-major, 128-byte swizzle).  The epilogue rounds the
+// accumulator to bf16, writes it into a double-buffered smem tile in the swizzled layout and stores it with one TMA
+// bulk store per warpgroup and 64 columns.
+//
+// Statistics, bit-identical to bn_stats_kernel's on the same y.  The row ranges of the CTAs are those of the
+// statistics pass (bn_stats_plan: a chunk is a multiple of 256 rows, so whole tiles), and the 256 consumer threads read
+// the staged bf16 tile back from smem in that kernel's thread layout -- thread (v, rl) takes channels 8v .. 8v+7 of each
+// 64-channel slab in rows rl, rl + 32, ... in increasing order -- and add (y - y[0, c]) and its square in the same fp32
+// order.  The per-CTA partials and the fixed-order fp64 finish in the last CTA of a slab are bn_stats_kernel's own
+// (bn_reduce.cuh), on named barriers of the consumer threads.  y[0, c], the shift, is computed by every CTA: the CTAs
+// after the first run tile 0 once more, without storing it.
+#include <cuda.h>
+#include <cuda_bf16.h>
+
+#include "../../include/moco_b200.h"
+#include "bn_reduce.cuh"
+#include "common.cuh"
+#include "sm90_ptx.cuh"
+#include "tc_common.cuh"
+
+namespace moco {
+
+constexpr int kCvThreads = 384;            // 2 consumer warpgroups + 1 producer warpgroup (one TMA thread)
+constexpr int kCvBM = 128;                 // rows per tile
+constexpr int kCvMaxSlabs = 64;            // 64-channel slabs (one ticket counter each in the workspace's 256 bytes)
+constexpr int kCvMaxPartials = 528;        // workspace sizing: slabs x CTAs per slab of the statistics plan
+static_assert(kBnStatsUnroll * kBnRows % kCvBM == 0, "a statistics chunk must be whole tiles");
+static_assert(kBnThreads == 256, "the consumer warpgroups are the statistics pass's threads");
+
+struct Conv1x1Args {
+    int M, Cin, m_tiles, ppc, R, stages;   // ppc = tiles per CTA; R = CTAs per column slice
+    float momentum, eps;
+    float* partial;                        // [slabs][R][128], bn_stats_kernel's layout
+    unsigned int* counters;                // [slabs]
+    float* mean;
+    float* invstd;
+    float* running_mean;                   // nullable (with running_var)
+    float* running_var;
+    long long* num_batches_tracked;        // nullable
+};
+
+template <int BN>
+struct Conv1x1Shape {
+    static constexpr int kA = kCvBM * 128;                 // x slab [128 rows x 64 bf16]
+    static constexpr int kB = BN * 128;                    // w slab [BN rows x 64 bf16]
+    static constexpr int kStage = kA + kB;
+    static constexpr int kOut = 64 * BN * 2;               // one warpgroup's [64 x BN] bf16 output tile
+    static constexpr int kP = 2 * kBnSlab;                 // floats of a slab partial: two sums per channel
+    // output buffers, shift, slab_reduce scratch, slab_finish totals
+    static constexpr int kFixed = 4 * kOut + BN * 4 + 8 * kP * 4 + 8 * kP * 8;
+};
+
+// the barrier of the two consumer warpgroups
+struct ConsumerSync {
+    __device__ __forceinline__ void operator()() const { named_bar_sync(3, kBnThreads); }
+};
+
+template <int BN>
+__global__ void __launch_bounds__(kCvThreads, 1)
+conv1x1_stats_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w,
+                     const __grid_constant__ CUtensorMap tm_y, const Conv1x1Args a) {
+    using S = Conv1x1Shape<BN>;
+    constexpr int kSlabs = BN / kBnSlab;
+    extern __shared__ __align__(1024) uint8_t smem[];
+    if ((smem_u32(smem) & 1023u) != 0u) __trap();
+    const int NS = a.stages;
+    uint8_t* ring = smem;                                          // NS x (x slab, w slab)
+    uint8_t* outb = ring + (size_t)NS * S::kStage;                 // [buffer][warpgroup] output tiles
+    float* shift_s = reinterpret_cast<float*>(outb + 4 * S::kOut); // [BN] y[0, c]
+    float* red = shift_s + BN;                                     // [8 warps][kP]
+    double* tot = reinterpret_cast<double*>(red + 8 * S::kP);      // [8 warps][kP]
+    uint64_t* full = reinterpret_cast<uint64_t*>(tot + 8 * S::kP);
+    uint64_t* empty = full + NS;
+    int* last = reinterpret_cast<int*>(empty + NS);
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int nb = blockIdx.x, r = blockIdx.y;
+    const int t0 = r * a.ppc;
+    const int t1 = min(t0 + a.ppc, a.m_tiles);
+    const int first = t0 > 0 ? -1 : 0;                             // iteration -1: tile 0 again, for the shift
+    const int ksteps = a.Cin >> 6;
+
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&tm_x);
+        tma_prefetch_desc(&tm_w);
+        tma_prefetch_desc(&tm_y);
+        for (int s = 0; s < NS; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
+        fence_mbar_init();
+    }
+    __syncthreads();
+
+    if (warp >= 8) {
+        setmaxnreg_dec<40>();
+        if (warp == 8 && elect_one()) {
+            // ---------------------------------------------------- TMA producer
+            int st = 0;
+            uint32_t ph = 0;
+            for (int it = first; it < t1 - t0; ++it) {
+                const int tile = it < 0 ? 0 : t0 + it;
+                for (int kc = 0; kc < ksteps; ++kc) {
+                    mbar_wait(&empty[st], ph ^ 1u);
+                    mbar_arrive_expect_tx(&full[st], (uint32_t)S::kStage);   // OOB rows count too (zero-filled)
+                    uint8_t* s = ring + (size_t)st * S::kStage;
+                    tma_load_2d(&tm_x, &full[st], s, kc * 64, tile * kCvBM);
+                    tma_load_2d(&tm_w, &full[st], s + S::kA, kc * 64, nb * BN);
+                    if (++st == NS) { st = 0; ph ^= 1u; }
+                }
+            }
+        }
+        return;
+    }
+    // ------------------------------------------------------------ consumer warpgroups
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2, t = threadIdx.x & 127;
+    const int rloc = (warp & 3) * 16 + (lane >> 2);               // rows rloc and rloc + 8 of the warpgroup's 64
+    const int ccol = 2 * (lane & 3);                              // first of this thread's two columns per 8
+    const int v = threadIdx.x & (kBnLanes - 1), rl = threadIdx.x >> 3;   // bn_stats_kernel's thread layout
+    const uint64_t a_desc0 = make_sw128_desc(smem_u32(ring + wg * 64 * 128), 16, 1024);
+    const uint64_t b_desc0 = make_sw128_desc(smem_u32(ring + S::kA), 16, 1024);
+    constexpr uint64_t kStageUnits = S::kStage >> 4;
+    float acc[BN / 2];
+    float sacc[kSlabs][16];                                       // per slab: 8 sums of (y - h), 8 of (y - h)^2
+    float sh[kSlabs][8];
+#pragma unroll
+    for (int s = 0; s < kSlabs; ++s)
+#pragma unroll
+        for (int k = 0; k < 16; ++k) sacc[s][k] = 0.f;
+    int st = 0;
+    uint32_t ph = 0;
+    for (int it = first; it < t1 - t0; ++it) {
+        const int tile = it < 0 ? 0 : t0 + it;
+        int prev = 0;
+        for (int kc = 0; kc < ksteps; ++kc) {
+            mbar_wait(&full[st], ph);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+                wgmma_ss<BN>(acc, a_desc0 + st * kStageUnits + 2 * k, b_desc0 + st * kStageUnits + 2 * k,
+                             (kc | k) != 0);
+            wgmma_commit();
+            wgmma_wait<1>();                                      // the previous chunk's wgmmas have completed
+            if (kc > 0 && t == 0) mbar_arrive(&empty[prev]);
+            prev = st;
+            if (++st == NS) { st = 0; ph ^= 1u; }
+        }
+        wgmma_wait<0>();
+        reg_fence(acc);
+        if (t == 0) mbar_arrive(&empty[prev]);
+
+        if (it == first) {                                        // tile 0: the shift y[0, c], as rounded
+            if (wg == 0 && warp == 0 && lane < 4) {
+#pragma unroll
+                for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e)
+                        shift_s[8 * j + ccol + e] = __bfloat162float(__float2bfloat16_rn(acc[4 * j + e]));
+            }
+            named_bar_sync(3, kBnThreads);
+#pragma unroll
+            for (int s = 0; s < kSlabs; ++s)
+#pragma unroll
+                for (int k = 0; k < 8; ++k) sh[s][k] = shift_s[s * kBnSlab + v * 8 + k];
+            if (it < 0) continue;
+        }
+
+        // ---- epilogue: bf16 tile -> smem -> TMA store, and the statistics read back from the staged tile
+        uint8_t* buf = outb + (it & 1) * 2 * S::kOut;             // [warpgroup] halves of this tile
+        uint8_t* ob = buf + wg * S::kOut;
+        if (t == 0) bulk_wait_read<1>();                          // the store that last used this buffer has read it
+        named_bar_sync(1 + wg, 128);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = rloc + 8 * h;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                const __nv_bfloat162 q = __floats2bfloat162_rn(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+                *reinterpret_cast<__nv_bfloat162*>(ob + (j >> 3) * 8192 + row * 128 + (((j & 7) ^ (row & 7)) << 4) +
+                                                   (lane & 3) * 4) = q;
+            }
+        }
+        fence_proxy_async();                                      // generic smem writes -> visible to the TMA store
+        named_bar_sync(3, kBnThreads);                            // both halves staged (and the buffer's last readers done)
+        if (t == 0) {
+#pragma unroll
+            for (int sl = 0; sl < BN / 64; ++sl)
+                tma_store_2d(&tm_y, ob + sl * 8192, nb * BN + sl * 64, tile * kCvBM + wg * 64);
+            bulk_commit();
+        }
+#pragma unroll
+        for (int p = 0; p < kCvBM / kBnRows; ++p) {
+            const int row = p * kBnRows + rl;
+            if (tile * kCvBM + row < a.M) {
+                const int lr = row & 63;
+                const uint8_t* src = buf + (row >> 6) * S::kOut + lr * 128 + ((v ^ (lr & 7)) << 4);
+#pragma unroll
+                for (int s = 0; s < kSlabs; ++s) {
+                    float f[8];
+                    unpack8(*reinterpret_cast<const uint4*>(src + s * 8192), f);
+#pragma unroll
+                    for (int k = 0; k < 8; ++k) {
+                        const float d = f[k] - sh[s][k];
+                        sacc[s][k] += d;
+                        sacc[s][8 + k] = fmaf(d, d, sacc[s][8 + k]);
+                    }
+                }
+            }
+        }
+    }
+    if (t == 0) bulk_wait<0>();
+
+    // ---- bn_stats_kernel's partials and finish, slab by slab
+#pragma unroll
+    for (int s = 0; s < kSlabs; ++s) {
+        const int gs = nb * kSlabs + s;
+        const float part = slab_reduce<2>(sacc[s], red, ConsumerSync());
+        if (slab_finish<2>(part, a.partial, a.counters + gs, gs, r, a.R, tot, last, ConsumerSync())) {
+            if (threadIdx.x < kBnSlab)
+                bn_stats_channel(tot, threadIdx.x, shift_s[s * kBnSlab + threadIdx.x], a.M, a.eps, a.momentum,
+                                 gs * kBnSlab + threadIdx.x, a.mean, a.invstd, a.running_mean, a.running_var);
+            if (gs == 0 && threadIdx.x == 0 && a.num_batches_tracked != nullptr) *a.num_batches_tracked += 1;
+        }
+        named_bar_sync(3, kBnThreads);                            // red / tot are reused by the next slab
+    }
+}
+
+size_t conv1x1_workspace_bytes() { return 256 + (size_t)kCvMaxPartials * 2 * kBnSlab * sizeof(float); }
+
+template <int BN>
+static cudaError_t launch_bn(const void* x, const void* w, void* y, int M, int Cin, int Cout, const BnLayer& bn,
+                             void* ws, cudaStream_t stream) {
+    using S = Conv1x1Shape<BN>;
+    Conv1x1Args a{};
+    a.M = M; a.Cin = Cin;
+    a.m_tiles = (M + kCvBM - 1) / kCvBM;
+    long long passes = 0, ppc = 0;
+    bn_stats_plan(M, Cout, &passes, &ppc, &a.R);           // the statistics pass's row chunks
+    a.ppc = (int)(ppc * kBnRows / kCvBM);
+    const int slices = Cout / BN, slabs = Cout / kBnSlab;
+    if (slabs > kCvMaxSlabs || (long long)slabs * a.R > kCvMaxPartials) return cudaErrorNotSupported;
+    constexpr int kBarBytes = 256;
+    int stages = (kSmemBudget - S::kFixed - kBarBytes) / S::kStage;
+    if (stages > 8) stages = 8;
+    a.stages = stages;
+    const int smem = stages * S::kStage + S::kFixed + kBarBytes;
+    a.momentum = bn.momentum; a.eps = bn.eps;
+    a.counters = static_cast<unsigned int*>(ws);
+    a.partial = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 256);
+    a.mean = bn.save_mean; a.invstd = bn.save_invstd;
+    a.running_mean = bn.running_mean; a.running_var = bn.running_var; a.num_batches_tracked = bn.num_batches_tracked;
+    CUtensorMap tm_x, tm_w, tm_y;
+    if (!make_tmap(&tm_x, x, M, Cin, kCvBM) || !make_tmap(&tm_w, w, Cout, Cin, BN) || !make_tmap(&tm_y, y, M, Cout, 64))
+        return cudaErrorUnknown;
+    {
+        std::lock_guard<std::mutex> lock(g_kernel_cache_mutex);
+        KernelCache& kc = kernel_cache(BN / 64 - 1);
+        if (kc.smem_set < smem) {
+            cudaError_t e = cudaFuncSetAttribute(conv1x1_stats_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                 smem);
+            if (e != cudaSuccess) return e;
+            kc.smem_set = smem;
+        }
+    }
+    conv1x1_stats_kernel<BN><<<dim3(slices, a.R), kCvThreads, smem, stream>>>(tm_x, tm_w, tm_y, a);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_conv1x1_bn_stats(const void* x, const void* w, void* y, long long M, int Cin, int Cout,
+                                    const BnLayer& bn, void* ws, cudaStream_t stream) {
+    if (M < 1 || M > 0x7fffff80LL || Cin < 64 || Cin % 64 != 0 || Cin > 65536 || Cout < 64 || Cout % 64 != 0 ||
+        Cout > 4096)
+        return cudaErrorNotSupported;
+    if (Cout % 128 == 0) return launch_bn<128>(x, w, y, (int)M, Cin, Cout, bn, ws, stream);
+    return launch_bn<64>(x, w, y, (int)M, Cin, Cout, bn, ws, stream);
+}
+
+}  // namespace moco

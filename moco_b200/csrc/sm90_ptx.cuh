@@ -116,6 +116,21 @@ __device__ __forceinline__ void tma_load_2d_mc(const void* tmap, uint64_t* bar, 
         : "memory");
 }
 
+// 2-D tile store from this CTA's smem (same box and swizzle as the map's loads); rows / columns outside the tensor are
+// not written.  Completion is tracked per issuing thread by bulk groups.
+__device__ __forceinline__ void tma_store_2d(const void* tmap, const void* src, int32_t c0, int32_t c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                 ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(src)), "r"(c0), "r"(c1)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still reading their smem source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// at most N of this thread's bulk groups not yet complete
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+
 // ---------------------------------------------------------------- wgmma
 // Register re-allocation between the warpgroups of a CTA (all warps of a warpgroup execute it).
 template <int R>

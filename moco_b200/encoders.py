@@ -59,13 +59,18 @@ class _Bottleneck(nn.Module):
             self.short = nn.Sequential(nn.Conv2d(cin, cout, 1, stride, bias=False), BatchNormAct2d(cout))
 
     def forward(self, x, avgpool=False):
-        """``avgpool``: return the global average pool of the output, [N, C] (the last block of the trunk)."""
-        y = self.bn1(self.conv1(x))
+        """``avgpool``: return the global average pool of the output, [N, C] (the last block of the trunk).  The 1x1
+        convolutions take the following BatchNorm's batch statistics with them where they can (bn.conv1x1_stats)."""
+        h, st = bn_mod.conv1x1_stats(self.conv1, self.bn1, x)
+        y = self.bn1(h, stats=st)
         y = self.bn2(self.conv2(y))
         r = bn_mod.hand_over(x)                   # x's second consumer: its gradient is summed in x's producer
         if self.short is None:
-            return self.bn3(self.conv3(y), r, avgpool=avgpool)
-        return self.bn3(self.conv3(y), self.short[0](r), shortcut_bn=self.short[1], avgpool=avgpool)   # one BN group
+            h, st = bn_mod.conv1x1_stats(self.conv3, self.bn3, y, r)
+            return self.bn3(h, r, avgpool=avgpool, stats=st)
+        s, sc_st = bn_mod.conv1x1_stats(self.short[0], self.short[1], r)
+        h, st = bn_mod.conv1x1_stats(self.conv3, self.bn3, y, s, self.short[1])
+        return self.bn3(h, s, shortcut_bn=self.short[1], avgpool=avgpool, stats=st, sc_stats=sc_st)   # one BN group
 
 
 class StemConv(nn.Conv2d):

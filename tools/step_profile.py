@@ -21,6 +21,7 @@ if ROOT not in sys.path:
 
 # (class, substrings of the kernel name); the first class with a matching substring wins
 CLASSES = [
+    ("conv1x1_stats", ("conv1x1_stats_kernel",)),     # csrc/conv1x1_sm90.cu: 1x1 forward + the next BN's statistics
     ("bn_stats", ("bn_stats_kernel",)),
     ("bn_apply", ("bn_apply_kernel",)),
     ("bn_bwd_reduce", ("bn_bwd_reduce_kernel",)),
