@@ -365,6 +365,30 @@ size_t moco_conv1x1_workspace_bytes(void);
 int moco_conv1x1_bn_stats(const void* x, const void* w, void* y, long long M, int Cin, int Cout,
                           const moco_bn_layer* bn, void* workspace, size_t workspace_bytes, void* stream);
 
+/* The backward of that convolution when its input is the output of a block's residual BatchNorm (moco_bn_add_relu_*,
+ * identity shortcut) whose gradient also has a second part dy2 (the next block's residual branch): the input gradient
+ * of the convolution taken with that BatchNorm's backward reduction.  One launch; deterministic.
+ *   dX = dh . w  (dh: bf16 [M, Cout], the gradient of the convolution's output; fp32 accumulation, rounded to bf16),
+ *   g  = mask . bf16(dX + dy2)   -- the masked gradient moco_bn_add_relu_bwd2 forms from dy = dX and dy2,
+ *   bn->dbeta = sum g,  bn->dgamma = sum g * x^   -- bit-identical to moco_bn_add_relu_bwd2's given the same dX.
+ * g (bf16 [M, Cin]) is written: it is also the residual gradient of an identity block.  Follow it with
+ * moco_bn_bwd_apply_given.  x: that BatchNorm's input, bf16 [M, Cin]; mask: its forward's mask bytes (uint8
+ * [M, Cin / 8]); only bn's save_mean, save_invstd, dgamma and dbeta are used.  Cin a power of two in [128, 2048],
+ * Cout a multiple of 64 in [64, 4096], 1 <= M < 2^31 - 128; pointers 16-byte aligned.  mask and dy2 are required
+ * and x2 / shortcut must be NULL: the other producers (a downsample block's bn3, a BatchNorm without residual) are
+ * MOCO_ERR_UNSUPPORTED.  workspace as for moco_conv1x1_bn_stats. */
+int moco_conv1x1_dgrad_bn_bwd(const void* dh, const void* w, void* g, long long M, int Cin, int Cout, const void* x,
+                              const void* mask, const void* dy2, const void* x2_or_null,
+                              const moco_bn_layer* bn, const moco_bn_layer* shortcut_or_null, void* workspace,
+                              size_t workspace_bytes, void* stream);
+/* The element-wise pass of the BatchNorm backward alone, on an already-masked gradient g whose sums are in bn->dbeta /
+ * bn->dgamma: dx as moco_bn_bwd.  Bit-identical to the second pass of moco_bn_add_relu_bwd(2) given the same g and
+ * sums.  One launch, no workspace.  g, x, dx: bf16 [M, C], 16-byte aligned, C a power of two in [64, 2048].  A shortcut
+ * BN (x2, dx2, shortcut) is validated but not implemented: MOCO_ERR_UNSUPPORTED. */
+int moco_bn_bwd_apply_given(const void* g, const void* x, const void* x2_or_null, long long M, int C,
+                            const moco_bn_layer* bn, const moco_bn_layer* shortcut_or_null, void* dx,
+                            void* dx2_or_null, void* stream);
+
 /* The stem's BatchNorm + ReLU followed by its 3x3 / stride 2 / pad 1 max pooling, without writing the BatchNorm's
  * output: bit-identical to moco_bn_fwd_train (relu = 1, no residual) + moco_maxpool3x3s2_fwd.  The statistics pass,
  * then one pass that applies BatchNorm + ReLU to every tap (rounded to bf16 as the BatchNorm's own pass stores it)

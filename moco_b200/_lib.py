@@ -81,6 +81,11 @@ SIGNATURES = {
     "moco_conv1x1_workspace_bytes": (c_size_t, []),
     "moco_conv1x1_bn_stats": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, POINTER(BnLayer), c_void_p,
                                       c_size_t, c_void_p]),
+    "moco_conv1x1_dgrad_bn_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p,
+                                          c_void_p, c_void_p, POINTER(BnLayer), POINTER(BnLayer), c_void_p, c_size_t,
+                                          c_void_p]),
+    "moco_bn_bwd_apply_given": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, POINTER(BnLayer),
+                                        POINTER(BnLayer), c_void_p, c_void_p, c_void_p]),
     "moco_bn_relu_maxpool_fwd_train": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
                                                POINTER(BnLayer), c_void_p, c_size_t, c_void_p]),
     "moco_bn_eval_act": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p, c_void_p, c_int, c_void_p,
@@ -142,7 +147,7 @@ class _Counting:
 
     _PER_CALL = {"moco_nce_shard_stats": 3, "moco_nce_shard_merge": 1, "moco_nce_shard_dq": 2,
                  "moco_nce_shard_dq_finish": 1, "moco_nce_shard_dq_finish_peers": 1, "moco_queue_enqueue_shard": 1, "moco_queue_enqueue": 1, "moco_f32_to_bf16": 1, "moco_shuffle_gather": 1, "moco_shuffle_gather_sync": 1, "moco_crop_gather_nhwc_bf16": 1,
-                 "moco_ema_update": 1, "moco_crop_to_nhwc_bf16": 1, "moco_bn_fwd_train": 2, "moco_bn_bwd": 2, "moco_bn_add_relu_bwd": 2, "moco_bn_add_relu_bwd2": 2, "moco_bn_relu_maxpool_fwd_train": 2, "moco_bn_eval_act": 1, "moco_bn_relu_maxpool_eval": 1, "moco_bn_eval_act_avgpool": 1, "moco_crop_s2d_bf16": 1, "moco_conv1x1_bn_stats": 1, "moco_maxpool3x3s2_fwd": 1, "moco_maxpool3x3s2_bwd": 1, "moco_maxpool3x3s2_bwd2": 1,
+                 "moco_ema_update": 1, "moco_crop_to_nhwc_bf16": 1, "moco_bn_fwd_train": 2, "moco_bn_bwd": 2, "moco_bn_add_relu_bwd": 2, "moco_bn_add_relu_bwd2": 2, "moco_bn_relu_maxpool_fwd_train": 2, "moco_bn_eval_act": 1, "moco_bn_relu_maxpool_eval": 1, "moco_bn_eval_act_avgpool": 1, "moco_crop_s2d_bf16": 1, "moco_conv1x1_bn_stats": 1, "moco_conv1x1_dgrad_bn_bwd": 1, "moco_bn_bwd_apply_given": 1, "moco_maxpool3x3s2_fwd": 1, "moco_maxpool3x3s2_bwd": 1, "moco_maxpool3x3s2_bwd2": 1,
                  "moco_signal_barrier": 1, "moco_nce_bwd_dense": 1}
 
     def __init__(self, lib):
@@ -252,8 +257,10 @@ def dtype_code(t) -> int:
 
 
 def cur_stream() -> int:
+    """torch.cuda.current_stream().cuda_stream of the current device, read without building a Stream object: it is
+    called for every launch, and the Stream path's device-index helpers cost more host time than most launches."""
     import torch
-    return torch.cuda.current_stream().cuda_stream
+    return torch._C._cuda_getCurrentRawStream(torch._C._cuda_getDevice())
 
 
 def require_cuda(*tensors) -> None:

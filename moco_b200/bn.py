@@ -59,7 +59,7 @@ def set_fused(flag: bool) -> None:
 
 def _workspace(device, conv=False):
     """The stream's workspace of the BatchNorm entry points, or (conv=True) of moco_conv1x1_bn_stats."""
-    key = (device.index, torch.cuda.current_stream(device).cuda_stream, conv)
+    key = (device.index, torch._C._cuda_getCurrentRawStream(device.index), conv)   # as _lib.cur_stream
     ws = _workspaces.get(key)
     if ws is None:
         lib = _lib.load()
@@ -221,8 +221,20 @@ class _BatchNormAddReluFn(torch.autograd.Function):
         N, C, H, W = x.shape
         M = N * H * W
         dy = _grad_rows(dy)
-        dy2 = _take_handed(ctx)          # y's other consumer's gradient: summed inside both passes
         dx = torch.empty_like(x)
+        reduced, ctx.reduced = getattr(ctx, "reduced", None), None
+        if reduced is not None and dy.data_ptr() == reduced[0].data_ptr():
+            # the consumer's dgrad formed g = dy and the sums (_dgrad_bn_bwd); another consumer adding to the gradient
+            # gives a different tensor, which takes the full backward below (g is already masked: mask(g + e) = g +
+            # mask(e))
+            g, dgamma, dbeta = reduced
+            bn = _layer(weight, None, mean, invstd, dgamma=dgamma, dbeta=dbeta)
+            # algorithmic bytes: reads g and x, writes dx
+            code = _timed("bn_bwd", M * C * 2 * 3, lambda: lib.moco_bn_bwd_apply_given(
+                g.data_ptr(), x.data_ptr(), None, M, C, bn, None, dx.data_ptr(), None, _lib.cur_stream()))
+            _lib.check(code, "moco_bn_bwd_apply_given")
+            return dx, g if ctx.needs_input_grad[1] else None, dgamma, dbeta, None, None, None, None, None, None, None
+        dy2 = _take_handed(ctx)          # y's other consumer's gradient: summed inside both passes
         f32 = lambda: torch.empty(C, dtype=torch.float32, device=x.device)
         dgamma, dbeta = f32(), f32()
         bn = _layer(weight, None, mean, invstd, dgamma=dgamma, dbeta=dbeta)
@@ -341,10 +353,11 @@ class _Conv1x1StatsFn(torch.autograd.Function):
     [Cout, Cin, 1, 1]) and the batch statistics of the training BatchNorm that reads y: one launch of
     ``moco_conv1x1_bn_stats``, which also updates that BatchNorm's running statistics.  Returns (y, mean, invstd).
     The backward is the convolution's own, ``aten.convolution_backward`` with the arguments autograd gives it for
-    ``F.conv2d``, so the gradients of a given forward are unchanged."""
+    ``F.conv2d``, so the gradients of a given forward are unchanged.  ``producer``: x's producing node when it may
+    take the input gradient together with its BatchNorm's backward reduction (:func:`_dgrad_bn_bwd`)."""
 
     @staticmethod
-    def forward(ctx, x, w, stats):
+    def forward(ctx, x, w, stats, producer=None):
         lib = _lib.load()
         N, Cin, H, W = x.shape
         Cout = w.shape[0]
@@ -357,15 +370,58 @@ class _Conv1x1StatsFn(torch.autograd.Function):
                                              _lib.cur_stream()), "moco_conv1x1_bn_stats")
         ctx.save_for_backward(x, w)
         ctx.mark_non_differentiable(mean, invstd)
+        ctx.producer = producer
         return y, mean, invstd
 
     @staticmethod
     def backward(ctx, dy, _dmean, _dinvstd):
         x, w = ctx.saved_tensors
+        want_dx = ctx.needs_input_grad[0]
+        g = _dgrad_bn_bwd(ctx.producer, dy, w) if ctx.producer is not None and want_dx else None
         dx, dw, _ = torch.ops.aten.convolution_backward(
             dy, x, w, None, [1, 1], [0, 0], [1, 1], False, [0, 0], 1,
-            [ctx.needs_input_grad[0], ctx.needs_input_grad[1], False])
-        return dx, dw, None
+            [want_dx and g is None, ctx.needs_input_grad[1], False])
+        return g if g is not None else dx, dw, None, None
+
+
+# (Cin, Cout) of ResNet-50's 1x1 convolutions fed by an identity block's output on which moco_conv1x1_dgrad_bn_bwd +
+# the apply-only pass measured faster than cuDNN's dgrad + moco_bn_add_relu_bwd2 at batch 256: 1.37-1.43x on an H100
+# SXM at a 700 W power limit (tools/conv1x1_dgrad_times.py, results/conv1x1_dgrad_times_h100.json).  These are all
+# such shapes that also run their forward on moco_conv1x1_bn_stats (_CONV1X1_WINS).
+_DGRAD_WINS = frozenset({(256, 64), (256, 128), (512, 128), (512, 256)})
+
+
+def _dgrad_wins(M, Cin, Cout):
+    """The shapes moco_conv1x1_dgrad_bn_bwd was measured to win on (_DGRAD_WINS) at batch 256's row counts."""
+    return M >= 50176 and (Cin, Cout) in _DGRAD_WINS
+
+
+def _dgrad_bn_bwd(node, dh, w):
+    """The input gradient of a 1x1 convolution whose input is the output of ``node``, a block's residual BatchNorm
+    (_BatchNormAddReluFn, identity shortcut), taken together with that BatchNorm's backward reduction: one launch of
+    moco_conv1x1_dgrad_bn_bwd forms g = mask . bf16(dX + dy2) -- dy2 the gradient the hand-over left on the node --
+    and the sums, and leaves (g, dgamma, dbeta) on the node for its backward (apply pass only).  None, to take
+    cuDNN's dgrad, when there is no handed gradient, the block has a shortcut BN, or the shape is not in _DGRAD_WINS."""
+    if getattr(node, "handed", None) is None:
+        return None
+    x, _, mask, weight, mean, invstd, sc_weight, _, _ = node.saved_tensors
+    N, C, H, W = x.shape
+    M, Cout = N * H * W, w.shape[0]
+    if mask is None or sc_weight is not None or not _dgrad_wins(M, C, Cout):
+        return None
+    lib = _lib.load()
+    dy2 = _take_handed(node)
+    dh = _grad_rows(dh)
+    g = torch.empty_like(x)
+    dgamma = torch.empty(C, dtype=torch.float32, device=x.device)
+    dbeta = torch.empty_like(dgamma)
+    ws = _workspace(x.device, conv=True)
+    _lib.check(lib.moco_conv1x1_dgrad_bn_bwd(
+        dh.data_ptr(), w.data_ptr(), g.data_ptr(), M, C, Cout, x.data_ptr(), mask.data_ptr(), dy2.data_ptr(), None,
+        _layer(weight, None, mean, invstd, dgamma=dgamma, dbeta=dbeta), None, ws.data_ptr(), ws.numel(),
+        _lib.cur_stream()), "moco_conv1x1_dgrad_bn_bwd")
+    node.reduced = (g, dgamma, dbeta)
+    return g
 
 
 # (Cin, Cout) of ResNet-50's stride-1 1x1 convolutions on which moco_conv1x1_bn_stats + the apply pass measured more
@@ -407,15 +463,19 @@ def _conv1x1_ok(conv, bn, x, residual=None, shortcut_bn=None):
     return _conv1x1_wins(N * H * W, Cin, Cout)
 
 
-def conv1x1_stats(conv, bn, x, residual=None, shortcut_bn=None):
+def conv1x1_stats(conv, bn, x, residual=None, shortcut_bn=None, handed_over=False):
     """(conv(x), stats): stats = the batch statistics of the training BatchNorm ``bn`` on conv(x), computed with the
     convolution by moco_conv1x1_bn_stats (``bn``'s running statistics are updated), to be passed to ``bn(...,
     stats=stats)``; None where that kernel does not take the convolution (see :func:`_conv1x1_ok`), which then runs
-    as ``conv(x)``.  ``residual`` / ``shortcut_bn``: what ``bn`` will be called with."""
+    as ``conv(x)``.  ``residual`` / ``shortcut_bn``: what ``bn`` will be called with.  ``handed_over``: x's only
+    other consumer is ``hand_over(x)``; when x is a block's residual BatchNorm output, the backward may then take the
+    input gradient with that BatchNorm's reduction (:func:`_dgrad_bn_bwd`)."""
     if not _conv1x1_ok(conv, bn, x, residual, shortcut_bn):
         return conv(x), None
     w = conv.weight.to(torch.bfloat16).contiguous()     # outside the Function: its autograd gives the fp32 gradient
-    y, mean, invstd = _Conv1x1StatsFn.apply(x, w, bn._stats())
+    node = x.grad_fn if handed_over else None
+    producer = node if isinstance(node, _BatchNormAddReluFn._backward_cls) else None
+    y, mean, invstd = _Conv1x1StatsFn.apply(x, w, bn._stats(), producer)
     return y, (mean, invstd)
 
 

@@ -39,7 +39,6 @@ constexpr int kBnMaxPartial = 3 * kBnSlab;           // floats per CTA partial: 
 // (16-byte loads in flight per thread and operand, resident CTAs per SM) of each kernel; every grid is one resident
 // wave (tools/bn_kernel_times.py times the variants over the layers of ResNet-50).
 constexpr int kBnApplyUnroll = 8, kBnApplyCtas = 2;
-constexpr int kBnBwdReduceUnroll = 4, kBnBwdReduceCtas = 2;
 constexpr int kBnBwdApplyUnroll = 2, kBnBwdApplyCtas = 3;
 constexpr int kBnBwdApplyScUnroll = 2, kBnBwdApplyScCtas = 2;   // with the shortcut BN: 48 coefficients per thread
 constexpr int kBnBwdApplySumUnroll = 2, kBnBwdApplySumCtas = 2; // with a second gradient (dy2): spills at 3 CTAs / SM
@@ -322,16 +321,9 @@ bn_bwd_reduce_kernel(const BnBwdReduceArgs a) {
     }
     const float part = slab_reduce<S>(acc, red);
     if (!slab_finish<S>(part, a.partial, a.counters + slab, slab, r, a.R, tot, &flag)) return;
-    if (threadIdx.x < kBnSlab) {
-        const int c8 = threadIdx.x >> 3, k = threadIdx.x & 7;
-        const int c = slab * kBnSlab + threadIdx.x;
-        a.sum_dy[c] = (float)tot[c8 * 8 * S + k];
-        a.sum_dy_xhat[c] = (float)(tot[c8 * 8 * S + 8 + k] * (double)a.invstd[c]);
-        if constexpr (kShortcut) {
-            a.sum_dy2[c] = (float)tot[c8 * 8 * S + k];
-            a.sum_dy_xhat2[c] = (float)(tot[c8 * 8 * S + 16 + k] * (double)a.invstd2[c]);
-        }
-    }
+    if (threadIdx.x < kBnSlab)
+        bn_bwd_channel<S>(tot, threadIdx.x, slab * kBnSlab + threadIdx.x, a.invstd, a.sum_dy, a.sum_dy_xhat, a.invstd2,
+                          a.sum_dy2, a.sum_dy_xhat2);
 }
 
 struct BnBwdApplyArgs {
@@ -593,6 +585,10 @@ void bn_stats_plan(long long M, int C, long long* passes, long long* ppc, int* R
     bn_reduce_plan(M, C, kBnStatsUnroll, kBnStatsCtas, passes, ppc, R);
 }
 
+void bn_bwd_reduce_plan(long long M, int C, long long* passes, long long* ppc, int* R) {
+    bn_reduce_plan(M, C, kBnBwdReduceUnroll, kBnBwdReduceCtas, passes, ppc, R);
+}
+
 static int bn_apply_grid(long long V, int unroll, int ctas_per_sm) {
     long long g = (V + (long long)kBnThreads * unroll - 1) / ((long long)kBnThreads * unroll);
     if (g > kBnSms * ctas_per_sm) g = kBnSms * ctas_per_sm;
@@ -739,6 +735,20 @@ cudaError_t launch_bn_add_relu_bwd(const void* dy, const void* dy2, const void* 
     p.mean = bn.save_mean; p.invstd = bn.save_invstd; p.gamma = bn.gamma;
     p.sum_dy = bn.dbeta; p.sum_dy_xhat = bn.dgamma;
     return dy2 != nullptr ? add_relu_bwd<true>(s, p, sc, dres, stream) : add_relu_bwd<false>(s, p, sc, dres, stream);
+}
+
+cudaError_t launch_bn_bwd_apply_given(const void* g, const void* x, const void* x2, long long M, int C, const BnLayer& bn,
+                                      const BnLayer* sc, void* dx, void* dx2, cudaStream_t stream) {
+    // a shortcut BN (x2, dx2) is not taken: its apply kernel reads the mask bits (kShortcut), and
+    // moco_conv1x1_dgrad_bn_bwd does not produce a downsample block's g
+    (void)x2; (void)dx2;
+    if (!bn_shape_ok(M, C) || sc != nullptr) return cudaErrorNotSupported;
+    BnBwdApplyArgs p{};
+    p.dy = static_cast<const uint4*>(g); p.x = static_cast<const uint4*>(x); p.dx = static_cast<uint4*>(dx);
+    p.V = M * (C >> 3); p.C = C; p.mask = kMaskNone; p.inv_m = (float)(1.0 / (double)M);
+    p.mean = bn.save_mean; p.invstd = bn.save_invstd; p.gamma = bn.gamma;
+    p.sum_dy = bn.dbeta; p.sum_dy_xhat = bn.dgamma;
+    return run_bwd_apply<kBnBwdApplyUnroll, kBnBwdApplyCtas, false>(p, stream);
 }
 
 cudaError_t launch_bn_relu_maxpool_fwd(const void* x, void* y, void* taps, int N, int H, int W, int C, const BnLayer& bn,

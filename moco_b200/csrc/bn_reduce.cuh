@@ -13,6 +13,8 @@ constexpr int kBnLanes = kBnSlab / 8;                // 16-byte vectors per slab
 constexpr int kBnRows = kBnThreads / kBnLanes;       // rows per pass
 // (16-byte loads in flight per thread, resident CTAs per SM) of the statistics kernel; its row plan (bn_stats_plan)
 constexpr int kBnStatsUnroll = 8, kBnStatsCtas = 2;
+// the same of the backward reduction kernel; its row plan (bn_bwd_reduce_plan)
+constexpr int kBnBwdReduceUnroll = 4, kBnBwdReduceCtas = 2;
 
 // the barrier of the kBnThreads threads that reduce: the whole CTA unless the caller passes its own
 struct CtaSync {
@@ -123,6 +125,21 @@ __device__ __forceinline__ void bn_stats_channel(const double* tot, int j, float
         const double unbiased = M > 1 ? var * ((double)M / (double)(M - 1)) : var;
         running_mean[c] = (1.f - momentum) * running_mean[c] + momentum * mean;
         running_var[c] = (1.f - momentum) * running_var[c] + momentum * (float)unbiased;
+    }
+}
+
+// One channel's backward sums from the slab totals of slab_reduce<S> / slab_finish<S> (sum g, sum g (x - mean) and,
+// S = 3, sum g (x2 - mean2) in element j = threadIdx.x < 64 of the slab): dbeta = sum g, dgamma = invstd * sum
+// g (x - mean) in fp64, and with S = 3 the shortcut BN's pair (its dbeta is the same sum).
+template <int S>
+__device__ __forceinline__ void bn_bwd_channel(const double* tot, int j, int c, const float* invstd, float* dbeta,
+                                               float* dgamma, const float* invstd2, float* dbeta2, float* dgamma2) {
+    const int c8 = j >> 3, k = j & 7;
+    dbeta[c] = (float)tot[c8 * 8 * S + k];
+    dgamma[c] = (float)(tot[c8 * 8 * S + 8 + k] * (double)invstd[c]);
+    if constexpr (S == 3) {
+        dbeta2[c] = (float)tot[c8 * 8 * S + k];
+        dgamma2[c] = (float)(tot[c8 * 8 * S + 16 + k] * (double)invstd2[c]);
     }
 }
 

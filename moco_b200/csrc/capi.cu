@@ -666,6 +666,55 @@ int moco_conv1x1_bn_stats(const void* x, const void* w, void* y, long long M, in
     return MOCO_OK;
 }
 
+int moco_conv1x1_dgrad_bn_bwd(const void* dh, const void* w, void* g, long long M, int Cin, int Cout, const void* x,
+                              const void* mask, const void* dy2, const void* x2, const moco_bn_layer* bn,
+                              const moco_bn_layer* shortcut, void* workspace, size_t workspace_bytes, void* stream_) {
+    g_err[0] = 0;
+    if (!dh || !w || !g || !x || !workspace || !bn || !bn->save_mean || !bn->save_invstd || !bn->dgamma ||
+        !bn->dbeta || (x2 == nullptr) != (shortcut == nullptr) || misaligned16(dh) || misaligned16(w) ||
+        misaligned16(g) || misaligned16(x) || misaligned16(mask) || misaligned16(dy2) || misaligned16(x2) ||
+        misaligned16(workspace) || g == dh || g == x || g == dy2) {
+        set_error("moco_conv1x1_dgrad_bn_bwd: bad argument (null / misaligned pointer, g aliasing an input, x2 without "
+                  "the shortcut BN or the reverse)");
+        return MOCO_ERR_INVALID;
+    }
+    if (!mask || !dy2 || x2 || M < 1 || M > 0x7fffff80LL || Cin < 128 || Cin > 2048 || (Cin & (Cin - 1)) != 0 ||
+        Cout < 64 || Cout % 64 != 0 || Cout > 4096) {
+        set_error("moco_conv1x1_dgrad_bn_bwd: needs the mask bits and dy2 without a shortcut BN, 1 <= M < 2^31 - 128, "
+                  "Cin a power of two in [128, 2048] and Cout a multiple of 64 in [64, 4096] (M=%lld Cin=%d Cout=%d)",
+                  M, Cin, Cout);
+        return MOCO_ERR_UNSUPPORTED;
+    }
+    if (workspace_bytes < conv1x1_workspace_bytes()) {
+        set_error("moco_conv1x1_dgrad_bn_bwd: workspace too small");
+        return MOCO_ERR_WORKSPACE;
+    }
+    cudaError_t e = launch_conv1x1_dgrad_bn_bwd(dh, w, g, M, Cin, Cout, x, mask, dy2, *bn, workspace,
+                                                static_cast<cudaStream_t>(stream_));
+    if (e != cudaSuccess) return cuda_fail("moco_conv1x1_dgrad_bn_bwd", e);
+    return MOCO_OK;
+}
+
+int moco_bn_bwd_apply_given(const void* g, const void* x, const void* x2, long long M, int C, const moco_bn_layer* bn,
+                            const moco_bn_layer* shortcut, void* dx, void* dx2, void* stream_) {
+    g_err[0] = 0;
+    if (!g || !x || !dx || !bn_layer_bwd_ok(bn) || (shortcut && (!bn_layer_bwd_ok(shortcut) || !x2 || !dx2)) ||
+        misaligned16(g) || misaligned16(x) || misaligned16(x2) || misaligned16(dx) || misaligned16(dx2)) {
+        set_error("moco_bn_bwd_apply_given: bad argument (null / misaligned pointer; x2 and dx2 are required with a "
+                  "shortcut BN)");
+        return MOCO_ERR_INVALID;
+    }
+    cudaError_t e = launch_bn_bwd_apply_given(g, x, x2, M, C, *bn, shortcut, dx, dx2,
+                                              static_cast<cudaStream_t>(stream_));
+    if (e == cudaErrorNotSupported) {
+        set_error("moco_bn_bwd_apply_given: needs M >= 1, C a power of two in [64, 2048] and no shortcut BN "
+                  "(M=%lld C=%d)", M, C);
+        return MOCO_ERR_UNSUPPORTED;
+    }
+    if (e != cudaSuccess) return cuda_fail("batch-norm backward kernels", e);
+    return MOCO_OK;
+}
+
 int moco_bn_add_relu_bwd(const void* dy, const void* x, const void* residual, const void* mask, long long M, int C,
                          const moco_bn_layer* bn, const moco_bn_layer* shortcut, void* dx, void* dresidual,
                          void* workspace, size_t workspace_bytes, void* stream_) {

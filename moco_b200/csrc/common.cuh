@@ -151,9 +151,20 @@ cudaError_t launch_bn_relu_maxpool_eval(const void* x, void* y, int N, int H, in
                                         const float* shift, cudaStream_t stream);
 // rows of the statistics pass: passes of kBnRows rows, ppc passes per CTA (a multiple of kBnStatsUnroll), R CTAs
 void bn_stats_plan(long long M, int C, long long* passes, long long* ppc, int* R);
+// the same of the backward reduction pass (a multiple of kBnBwdReduceUnroll passes per CTA)
+void bn_bwd_reduce_plan(long long M, int C, long long* passes, long long* ppc, int* R);
+// the element-wise backward pass alone on an already-masked gradient g whose sums are in bn.dbeta / bn.dgamma (and
+// sc's): dx (and the shortcut BN's input gradient dx2)
+cudaError_t launch_bn_bwd_apply_given(const void* g, const void* x, const void* x2, long long M, int C, const BnLayer& bn,
+                                      const BnLayer* sc, void* dx, void* dx2, cudaStream_t stream);
 size_t conv1x1_workspace_bytes();
 cudaError_t launch_conv1x1_bn_stats(const void* x, const void* w, void* y, long long M, int Cin, int Cout,
                                     const BnLayer& bn, void* ws, cudaStream_t stream);
+// dgrad of a 1x1 convolution, g = mask . bf16(bf16(dH . w) + dy2), and the backward sums of the BatchNorm that
+// produced the convolution's input (moco_conv1x1_dgrad_bn_bwd)
+cudaError_t launch_conv1x1_dgrad_bn_bwd(const void* dh, const void* w, void* g, long long M, int Cin, int Cout,
+                                        const void* x, const void* mask, const void* dy2, const BnLayer& bn, void* ws,
+                                        cudaStream_t stream);
 int ema_chunk_elems();
 cudaError_t launch_ema(const void* segs, const int* chunk_prefix, int n_segs, int n_chunks, float m,
                        float one_minus_m, cudaStream_t stream);

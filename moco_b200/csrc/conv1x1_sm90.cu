@@ -284,4 +284,277 @@ cudaError_t launch_conv1x1_bn_stats(const void* x, const void* w, void* y, long 
     return launch_bn<64>(x, w, y, (int)M, Cin, Cout, bn, ws, stream);
 }
 
+// ---- backward: the input gradient with the producing BatchNorm's backward reduction ---------------------------------
+// The convolution's input is the output of a block's residual BatchNorm, y = relu(bn(x) + r), and it has a second
+// consumer, the next block's residual branch, whose gradient dy2 is handed over (bn.py: hand_over).  The dgrad GEMM
+//     dX[M, Cin] = dH[M, Cout] . w[Cout, Cin]                 (w as stored is the MN-major B operand: wgmma_ss_tb)
+// rounds dX to bf16 (what cuDNN's dgrad stores), adds dy2 with sum_grads' single rounding and applies the forward's
+// ReLU mask bits: g, the masked gradient that bn_bwd_reduce_kernel / bn_bwd_apply_kernel would form from the same
+// inputs.  g is written once (it is also the residual gradient of an identity block), and the reduction sums
+// sum g and sum g (x - mean) are taken from the staged tile in bn_bwd_reduce_kernel's row plan (bn_bwd_reduce_plan:
+// chunks of 128 rows, so whole tiles), thread layout and fp32 order, finished by its own code: bit-identical dbeta /
+// dgamma.  Only moco_bn_bwd_apply_given is left to run.
+// The epilogue operands (x, dy2 and the mask bytes of the tile's 128 columns: 66 KB per tile against 16-64 KB of
+// mainloop operands) are loaded by the TMA producer into two buffers, one tile ahead of the consumers.  g is staged in
+// place over dy2 and stored from there.
+constexpr int kDgBN = 128;                       // columns of dX per CTA
+struct DgradShape {
+    static constexpr int kA = kCvBM * 128;               // dH slab [128 rows x 64 bf16], K-major
+    static constexpr int kB = kDgBN * 128;               // w slab [64 K rows x 128 bf16], MN-major: two 64-column boxes
+    static constexpr int kStage = kA + kB;
+    static constexpr int kTile = 2 * kSlab;              // [2 column slabs][128 rows x 64 bf16], 128-byte swizzle
+    static constexpr int kMask = kCvBM * kDgBN / 8;      // [128 rows][16 mask bytes]
+    static constexpr int kEpi = 2 * kTile + kMask;       // x tile, dy2 tile (then g), mask bytes
+    static constexpr int kP = 2 * kBnSlab;
+    static constexpr int kFixed = 2 * kEpi + 8 * kP * 4 + 8 * kP * 8;
+};
+static_assert(kBnBwdReduceUnroll * kBnRows % kCvBM == 0, "a reduction chunk must be whole tiles");
+static_assert(DgradShape::kEpi % 1024 == 0, "epilogue buffers keep the 1024-byte alignment of the swizzled tiles");
+
+struct DgradArgs {
+    int M, K, m_tiles, ppc, R, stages;   // K = Cout; ppc = tiles per CTA; R = CTAs per column slice
+    float* partial;                      // [slabs][R][128], bn_bwd_reduce_kernel's layout
+    unsigned int* counters;              // [slabs]
+    const float* mean;
+    const float* invstd;
+    float* dgamma;
+    float* dbeta;
+};
+
+__global__ void __launch_bounds__(kCvThreads, 1)
+conv1x1_dgrad_bn_bwd_kernel(const __grid_constant__ CUtensorMap tm_dh, const __grid_constant__ CUtensorMap tm_w,
+                            const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_dy2,
+                            const __grid_constant__ CUtensorMap tm_mask, const __grid_constant__ CUtensorMap tm_g,
+                            const DgradArgs a) {
+    using S = DgradShape;
+    constexpr int kSlabs = kDgBN / kBnSlab;
+    extern __shared__ __align__(1024) uint8_t smem[];
+    if ((smem_u32(smem) & 1023u) != 0u) __trap();
+    const int NS = a.stages;
+    uint8_t* ring = smem;                                          // NS x (dH slab, w slab)
+    uint8_t* epi = ring + (size_t)NS * S::kStage;                  // [2] x (x tile, dy2 / g tile, mask bytes)
+    float* red = reinterpret_cast<float*>(epi + 2 * S::kEpi);      // [8 warps][kP]
+    double* tot = reinterpret_cast<double*>(red + 8 * S::kP);      // [8 warps][kP]
+    uint64_t* full = reinterpret_cast<uint64_t*>(tot + 8 * S::kP);
+    uint64_t* empty = full + NS;
+    uint64_t* efull = empty + NS;
+    uint64_t* eempty = efull + 2;
+    int* last = reinterpret_cast<int*>(eempty + 2);
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int nb = blockIdx.x, r = blockIdx.y;
+    const int t0 = r * a.ppc;
+    const int t1 = min(t0 + a.ppc, a.m_tiles);
+    const int ksteps = a.K >> 6;
+
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&tm_dh);
+        tma_prefetch_desc(&tm_w);
+        tma_prefetch_desc(&tm_x);
+        tma_prefetch_desc(&tm_dy2);
+        tma_prefetch_desc(&tm_mask);
+        tma_prefetch_desc(&tm_g);
+        for (int s = 0; s < NS; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
+        for (int b = 0; b < 2; ++b) { mbar_init(&efull[b], 1); mbar_init(&eempty[b], kBnThreads); }
+        fence_mbar_init();
+    }
+    __syncthreads();
+
+    if (warp >= 8) {
+        setmaxnreg_dec<40>();
+        if (warp == 8 && elect_one()) {
+            // ---------------------------------------------------- TMA producer
+            int st = 0;
+            uint32_t ph = 0;
+            for (int it = 0; it < t1 - t0; ++it) {
+                const int tile = t0 + it, eb = it & 1;
+                const int row0 = tile * kCvBM;
+                mbar_wait(&eempty[eb], ((it >> 1) & 1) ^ 1u);
+                mbar_arrive_expect_tx(&efull[eb], (uint32_t)S::kEpi);  // OOB rows count too (zero-filled)
+                uint8_t* e = epi + eb * S::kEpi;
+#pragma unroll
+                for (int s = 0; s < kSlabs; ++s) {
+                    tma_load_2d(&tm_x, &efull[eb], e + s * kSlab, nb * kDgBN + s * 64, row0);
+                    tma_load_2d(&tm_dy2, &efull[eb], e + S::kTile + s * kSlab, nb * kDgBN + s * 64, row0);
+                }
+                tma_load_2d(&tm_mask, &efull[eb], e + 2 * S::kTile, nb * (kDgBN / 8), row0);
+                for (int kc = 0; kc < ksteps; ++kc) {
+                    mbar_wait(&empty[st], ph ^ 1u);
+                    mbar_arrive_expect_tx(&full[st], (uint32_t)S::kStage);
+                    uint8_t* s = ring + (size_t)st * S::kStage;
+                    tma_load_2d(&tm_dh, &full[st], s, kc * 64, row0);
+                    tma_load_2d(&tm_w, &full[st], s + S::kA, nb * kDgBN, kc * 64);
+                    tma_load_2d(&tm_w, &full[st], s + S::kA + S::kB / 2, nb * kDgBN + 64, kc * 64);
+                    if (++st == NS) { st = 0; ph ^= 1u; }
+                }
+            }
+        }
+        return;
+    }
+    // ------------------------------------------------------------ consumer warpgroups
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2, t = threadIdx.x & 127;
+    const int rloc = wg * 64 + (warp & 3) * 16 + (lane >> 2);    // tile rows rloc and rloc + 8
+    const int ccol = 2 * (lane & 3);                              // first of this thread's two columns per 8
+    const int v = threadIdx.x & (kBnLanes - 1), rl = threadIdx.x >> 3;   // bn_bwd_reduce_kernel's thread layout
+    const uint64_t a_desc0 = make_sw128_desc(smem_u32(ring + wg * 64 * 128), 16, 1024);
+    const uint64_t b_desc0 = make_sw128_desc(smem_u32(ring + S::kA), S::kB / 2, 1024);
+    constexpr uint64_t kStageUnits = S::kStage >> 4;
+    float acc[kDgBN / 2];
+    float sacc[kSlabs][16];                                       // per slab: 8 sums of g, 8 of g (x - mean)
+    float mu[kSlabs][8];
+#pragma unroll
+    for (int s = 0; s < kSlabs; ++s)
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            mu[s][k] = __ldg(a.mean + nb * kDgBN + s * kBnSlab + v * 8 + k);
+            sacc[s][k] = sacc[s][8 + k] = 0.f;
+        }
+    int st = 0;
+    uint32_t ph = 0;
+    for (int it = 0; it < t1 - t0; ++it) {
+        const int tile = t0 + it, eb = it & 1;
+        int prev = 0;
+        for (int kc = 0; kc < ksteps; ++kc) {
+            mbar_wait(&full[st], ph);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+                wgmma_ss_tb<kDgBN>(acc, a_desc0 + st * kStageUnits + 2 * k, b_desc0 + st * kStageUnits + 128 * k,
+                                   (kc | k) != 0);
+            wgmma_commit();
+            wgmma_wait<1>();                                      // the previous chunk's wgmmas have completed
+            if (kc > 0 && t == 0) mbar_arrive(&empty[prev]);
+            prev = st;
+            if (++st == NS) { st = 0; ph ^= 1u; }
+        }
+        wgmma_wait<0>();
+        reg_fence(acc);
+        if (t == 0) mbar_arrive(&empty[prev]);
+
+        // ---- epilogue: g = mask . bf16(bf16(dX) + dy2), in place over dy2 -> TMA store; the sums from the staged tile
+        uint8_t* e = epi + eb * S::kEpi;
+        uint8_t* gt = e + S::kTile;
+        const uint8_t* mt = e + 2 * S::kTile;
+        mbar_wait(&efull[eb], (it >> 1) & 1);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = rloc + 8 * h;
+#pragma unroll
+            for (int j = 0; j < kDgBN / 8; ++j) {
+                __nv_bfloat162* p = reinterpret_cast<__nv_bfloat162*>(gt + (j >> 3) * kSlab + row * 128 +
+                                                                      (((j & 7) ^ (row & 7)) << 4) + (lane & 3) * 4);
+                const float2 d2 = __bfloat1622float2(*p);
+                const unsigned int bits = (unsigned int)mt[row * (kDgBN / 8) + j] >> ccol;
+                const float d0 = __bfloat162float(__float2bfloat16_rn(acc[4 * j + 2 * h]));
+                const float d1 = __bfloat162float(__float2bfloat16_rn(acc[4 * j + 2 * h + 1]));
+                const float g0 = __bfloat162float(__float2bfloat16_rn(__fadd_rn(d0, d2.x)));
+                const float g1 = __bfloat162float(__float2bfloat16_rn(__fadd_rn(d1, d2.y)));
+                *p = __floats2bfloat162_rn((bits & 1u) ? g0 : 0.f, (bits & 2u) ? g1 : 0.f);
+            }
+        }
+        fence_proxy_async();                                      // generic smem writes -> visible to the TMA store
+        named_bar_sync(3, kBnThreads);                            // the whole tile staged
+        if (threadIdx.x == 0) {
+#pragma unroll
+            for (int s = 0; s < kSlabs; ++s) tma_store_2d(&tm_g, gt + s * kSlab, nb * kDgBN + s * 64, tile * kCvBM);
+            bulk_commit();
+        }
+#pragma unroll
+        for (int p = 0; p < kCvBM / kBnRows; ++p) {
+            const int row = p * kBnRows + rl;
+            if (tile * kCvBM + row < a.M) {
+                const int off = row * 128 + ((v ^ (row & 7)) << 4);
+#pragma unroll
+                for (int s = 0; s < kSlabs; ++s) {
+                    float g[8], f[8];
+                    unpack8(*reinterpret_cast<const uint4*>(gt + s * kSlab + off), g);
+                    unpack8(*reinterpret_cast<const uint4*>(e + s * kSlab + off), f);
+#pragma unroll
+                    for (int k = 0; k < 8; ++k) {
+                        sacc[s][k] += g[k];
+                        sacc[s][8 + k] = fmaf(g[k], f[k] - mu[s][k], sacc[s][8 + k]);
+                    }
+                }
+            }
+        }
+        if (threadIdx.x == 0) bulk_wait_read<0>();               // the store has read g out of the buffer
+        mbar_arrive(&eempty[eb]);
+    }
+    if (threadIdx.x == 0) bulk_wait<0>();
+
+    // ---- bn_bwd_reduce_kernel's partials and finish, slab by slab
+#pragma unroll
+    for (int s = 0; s < kSlabs; ++s) {
+        const int gs = nb * kSlabs + s;
+        const float part = slab_reduce<2>(sacc[s], red, ConsumerSync());
+        if (slab_finish<2>(part, a.partial, a.counters + gs, gs, r, a.R, tot, last, ConsumerSync())) {
+            if (threadIdx.x < kBnSlab)
+                bn_bwd_channel<2>(tot, threadIdx.x, gs * kBnSlab + threadIdx.x, a.invstd, a.dbeta, a.dgamma, nullptr,
+                                  nullptr, nullptr);
+        }
+        named_bar_sync(3, kBnThreads);                            // red / tot are reused by the next slab
+    }
+}
+
+// [rows, cols] uint8 row-major tensor (the mask bytes), box = [box_rows, 16 bytes], no swizzle, OOB -> zeros
+static bool make_tmap_u8(CUtensorMap* m, const void* base, int rows, int cols, int box_rows) {
+    EncodeTiledFn fn = get_encode_fn();
+    if (!fn) { set_error("cuTensorMapEncodeTiled entry point not available"); return false; }
+    cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+    cuuint64_t strides[1] = {(cuuint64_t)cols};
+    cuuint32_t box[2] = {16u, (cuuint32_t)box_rows};
+    cuuint32_t estr[2] = {1u, 1u};
+    CUresult res = fn(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), dims, strides, box, estr,
+                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (res != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (CUresult %d)", (int)res); return false; }
+    return true;
+}
+
+cudaError_t launch_conv1x1_dgrad_bn_bwd(const void* dh, const void* w, void* g, long long M, int Cin, int Cout,
+                                        const void* x, const void* mask, const void* dy2, const BnLayer& bn, void* ws,
+                                        cudaStream_t stream) {
+    // Cin is the BatchNorm's C (a power of two in [128, 2048]); Cout the GEMM's K
+    if (M < 1 || M > 0x7fffff80LL || Cin < kDgBN || Cin > 2048 || (Cin & (Cin - 1)) != 0 || Cout < 64 ||
+        Cout % 64 != 0 || Cout > 4096)
+        return cudaErrorNotSupported;
+    using S = DgradShape;
+    DgradArgs a{};
+    a.M = (int)M; a.K = Cout;
+    a.m_tiles = (int)((M + kCvBM - 1) / kCvBM);
+    long long passes = 0, ppc = 0;
+    bn_bwd_reduce_plan(M, Cin, &passes, &ppc, &a.R);       // bn_bwd_reduce_kernel's row chunks
+    a.ppc = (int)(ppc * kBnRows / kCvBM);
+    const int slices = Cin / kDgBN, slabs = Cin / kBnSlab;
+    if ((long long)slabs * a.R > kCvMaxPartials) return cudaErrorNotSupported;
+    constexpr int kBarBytes = 256;
+    int stages = (kSmemBudget - S::kFixed - kBarBytes) / S::kStage;
+    if (stages > 8) stages = 8;
+    if (stages < 2) return cudaErrorNotSupported;
+    a.stages = stages;
+    const int smem = stages * S::kStage + S::kFixed + kBarBytes;
+    a.counters = static_cast<unsigned int*>(ws);
+    a.partial = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 256);
+    a.mean = bn.save_mean; a.invstd = bn.save_invstd; a.dgamma = bn.dgamma; a.dbeta = bn.dbeta;
+    CUtensorMap tm_dh, tm_w, tm_x, tm_dy2, tm_mask, tm_g;
+    if (!make_tmap(&tm_dh, dh, (int)M, Cout, kCvBM) || !make_tmap(&tm_w, w, Cout, Cin, 64) ||
+        !make_tmap(&tm_x, x, (int)M, Cin, kCvBM) || !make_tmap(&tm_dy2, dy2, (int)M, Cin, kCvBM) ||
+        !make_tmap_u8(&tm_mask, mask, (int)M, Cin / 8, kCvBM) || !make_tmap(&tm_g, g, (int)M, Cin, kCvBM))
+        return cudaErrorUnknown;
+    {
+        std::lock_guard<std::mutex> lock(g_kernel_cache_mutex);
+        KernelCache& kc = kernel_cache(2);
+        if (kc.smem_set < smem) {
+            cudaError_t e = cudaFuncSetAttribute(conv1x1_dgrad_bn_bwd_kernel,
+                                                 cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+            if (e != cudaSuccess) return e;
+            kc.smem_set = smem;
+        }
+    }
+    conv1x1_dgrad_bn_bwd_kernel<<<dim3(slices, a.R), kCvThreads, smem, stream>>>(tm_dh, tm_w, tm_x, tm_dy2, tm_mask,
+                                                                                  tm_g, a);
+    return cudaGetLastError();
+}
+
 }  // namespace moco

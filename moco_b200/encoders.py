@@ -61,7 +61,7 @@ class _Bottleneck(nn.Module):
     def forward(self, x, avgpool=False):
         """``avgpool``: return the global average pool of the output, [N, C] (the last block of the trunk).  The 1x1
         convolutions take the following BatchNorm's batch statistics with them where they can (bn.conv1x1_stats)."""
-        h, st = bn_mod.conv1x1_stats(self.conv1, self.bn1, x)
+        h, st = bn_mod.conv1x1_stats(self.conv1, self.bn1, x, handed_over=True)   # x's other consumer: hand_over
         y = self.bn1(h, stats=st)
         y = self.bn2(self.conv2(y))
         r = bn_mod.hand_over(x)                   # x's second consumer: its gradient is summed in x's producer

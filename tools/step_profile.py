@@ -22,6 +22,8 @@ if ROOT not in sys.path:
 # (class, substrings of the kernel name); the first class with a matching substring wins
 CLASSES = [
     ("conv1x1_stats", ("conv1x1_stats_kernel",)),     # csrc/conv1x1_sm90.cu: 1x1 forward + the next BN's statistics
+    # 1x1 dgrad + the producing BN's backward sums; before conv_dgrad, which takes any name containing "dgrad"
+    ("conv1x1_dgrad_bn", ("conv1x1_dgrad_bn_bwd_kernel",)),
     ("bn_stats", ("bn_stats_kernel",)),
     ("bn_apply", ("bn_apply_kernel",)),
     ("bn_bwd_reduce", ("bn_bwd_reduce_kernel",)),
