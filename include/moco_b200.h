@@ -365,6 +365,25 @@ size_t moco_conv1x1_workspace_bytes(void);
 int moco_conv1x1_bn_stats(const void* x, const void* w, void* y, long long M, int Cin, int Cout,
                           const moco_bn_layer* bn, void* workspace, size_t workspace_bytes, void* stream);
 
+/* A block's residual BatchNorm on that convolution's output, y = relu(bn(x . w^T) + r), computed from the convolution's
+ * INPUT x: the GEMM runs again with the BatchNorm, the add and the ReLU in its epilogue, so the convolution's output h
+ * is neither written nor read here.  r as in moco_bn_fwd_train_given (residual, or bf16(shortcut_bn(residual)) with a
+ * shortcut BN).  With the same statistics, y and the mask bits are bit-identical to moco_conv1x1_bn_stats followed by
+ * moco_bn_fwd_train_given (relu = 1): the recomputed tile is, by construction, the h that call stores.
+ *   stats_given bit MOCO_BN_STATS_GIVEN set: bn's statistics are final (moco_conv1x1_bn_stats ran; a backward that
+ *     needs h has it from there).  Clear: moco_conv1x1_bn_stats's pass runs first WITHOUT storing h -- for a forward
+ *     with no backward, where h is never needed.
+ *   MOCO_BN_SC_STATS_GIVEN clear with a shortcut BN: its statistics pass over residual runs first.
+ * x: bf16 [M, Cin], w: bf16 [Cout, Cin], residual, y: bf16 [M, Cout], mask (nullable): uint8 [M, Cout / 8]; pointers
+ * 16-byte aligned.  Cin a multiple of 64 in [64, 65536], Cout a power of two in [64, 2048], 1 <= M < 2^31 - 128.
+ * workspace: zeroed once, private to one stream, at least the larger of moco_conv1x1_workspace_bytes() and
+ * moco_bn_workspace_bytes() when a statistics pass runs (NULL otherwise allowed).  One launch plus one per statistics
+ * pass. */
+int moco_conv1x1_bn_add_relu_fwd(const void* x, const void* w, const void* residual, void* y, void* mask_or_null,
+                                 long long M, int Cin, int Cout, const moco_bn_layer* bn,
+                                 const moco_bn_layer* shortcut_or_null, int stats_given, void* workspace,
+                                 size_t workspace_bytes, void* stream);
+
 /* The backward of that convolution when its input is the output of a block's residual BatchNorm (moco_bn_add_relu_*,
  * identity shortcut) whose gradient also has a second part dy2 (the next block's residual branch): the input gradient
  * of the convolution taken with that BatchNorm's backward reduction.  One launch; deterministic.

@@ -81,6 +81,9 @@ SIGNATURES = {
     "moco_conv1x1_workspace_bytes": (c_size_t, []),
     "moco_conv1x1_bn_stats": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, POINTER(BnLayer), c_void_p,
                                       c_size_t, c_void_p]),
+    "moco_conv1x1_bn_add_relu_fwd": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int,
+                                             POINTER(BnLayer), POINTER(BnLayer), c_int, c_void_p, c_size_t,
+                                             c_void_p]),
     "moco_conv1x1_dgrad_bn_bwd": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p,
                                           c_void_p, c_void_p, POINTER(BnLayer), POINTER(BnLayer), c_void_p, c_size_t,
                                           c_void_p]),
@@ -165,6 +168,9 @@ class _Counting:
             elif name == "moco_bn_fwd_train_given":     # the apply pass + the statistics passes not given
                 setattr(self, name, self._wrap_count(fn, lambda a: 1 + (not a[9] & BN_STATS_GIVEN)
                                                      + (a[8] is not None and not a[9] & BN_SC_STATS_GIVEN)))
+            elif name == "moco_conv1x1_bn_add_relu_fwd":  # the same, with the GEMM's statistics pass
+                setattr(self, name, self._wrap_count(fn, lambda a: 1 + (not a[10] & BN_STATS_GIVEN)
+                                                     + (a[9] is not None and not a[10] & BN_SC_STATS_GIVEN)))
             elif name in self._PER_CALL:
                 setattr(self, name, self._wrap(fn, self._PER_CALL[name]))
             else:

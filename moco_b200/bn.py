@@ -175,10 +175,11 @@ class _BatchNormAddReluFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, x, residual, weight, bias, sc_weight, sc_bias, stats, sc_stats, want_mask, given=None,
-                sc_given=None):
+                sc_given=None, recompute=None):
         """given / sc_given: (mean, invstd) of the BatchNorm / the shortcut BN already computed by the producing
         convolution (:func:`conv1x1_stats`), which also updated its running statistics; that statistics pass is
-        skipped."""
+        skipped.  recompute: (a, w) with x = conv2d(a, w) of a 1x1 convolution (given required): y is computed from a
+        by moco_conv1x1_bn_add_relu_fwd instead of reading x (:func:`conv1x1_bn_add_relu`)."""
         lib = _lib.load()
         N, C, H, W = x.shape
         M = N * H * W
@@ -198,7 +199,16 @@ class _BatchNormAddReluFn(torch.autograd.Function):
         passes = (given is None) + (sc is not None and sc_given is None)
         nbytes = M * C * 2 * (3 + passes) + (M * C // 8 if want_mask else 0)
         mask_ptr = mask.data_ptr() if mask is not None else None
-        if flags:
+        if recompute is not None:
+            a, w = recompute
+            Cin = a.shape[1]
+            # algorithmic bytes: reads a, residual (+ the shortcut input for its statistics), writes y (+ mask bits)
+            nbytes = M * 2 * (Cin + C * (2 + passes)) + (M * C // 8 if want_mask else 0)
+            code = _timed("bn_fwd", nbytes, lambda: lib.moco_conv1x1_bn_add_relu_fwd(
+                a.data_ptr(), w.data_ptr(), residual.data_ptr(), y.data_ptr(), mask_ptr, M, Cin, C, bn, sc, flags,
+                ws.data_ptr(), ws.numel(), _lib.cur_stream()))
+            _lib.check(code, "moco_conv1x1_bn_add_relu_fwd")
+        elif flags:
             code = _timed("bn_fwd", nbytes, lambda: lib.moco_bn_fwd_train_given(
                 x.data_ptr(), residual.data_ptr(), y.data_ptr(), mask_ptr, M, C, 1, bn, sc, flags, ws.data_ptr(),
                 ws.numel(), _lib.cur_stream()))
@@ -233,7 +243,8 @@ class _BatchNormAddReluFn(torch.autograd.Function):
             code = _timed("bn_bwd", M * C * 2 * 3, lambda: lib.moco_bn_bwd_apply_given(
                 g.data_ptr(), x.data_ptr(), None, M, C, bn, None, dx.data_ptr(), None, _lib.cur_stream()))
             _lib.check(code, "moco_bn_bwd_apply_given")
-            return dx, g if ctx.needs_input_grad[1] else None, dgamma, dbeta, None, None, None, None, None, None, None
+            return (dx, g if ctx.needs_input_grad[1] else None, dgamma, dbeta, None, None, None, None, None, None, None,
+                    None)
         dy2 = _take_handed(ctx)          # y's other consumer's gradient: summed inside both passes
         f32 = lambda: torch.empty(C, dtype=torch.float32, device=x.device)
         dgamma, dbeta = f32(), f32()
@@ -261,7 +272,7 @@ class _BatchNormAddReluFn(torch.autograd.Function):
                 dy.data_ptr(), dy2.data_ptr(), x.data_ptr(), ptr(residual), mask.data_ptr(), M, C, bn, sc,
                 dx.data_ptr(), ptr(dres), ws.data_ptr(), ws.numel(), _lib.cur_stream()))
             _lib.check(code, "moco_bn_add_relu_bwd2")
-        return dx, dres, dgamma, dbeta, sc_dgamma, sc_dbeta, None, None, None, None, None
+        return dx, dres, dgamma, dbeta, sc_dgamma, sc_dbeta, None, None, None, None, None, None
 
 
 class _BatchNormReluMaxPoolFn(torch.autograd.Function):
@@ -479,6 +490,71 @@ def conv1x1_stats(conv, bn, x, residual=None, shortcut_bn=None, handed_over=Fals
     return y, (mean, invstd)
 
 
+# (Cin, Cout, key, shortcut) of ResNet-50's conv3 -> bn3 on which moco_conv1x1_bn_add_relu_fwd measured more than 3 %
+# faster than moco_conv1x1_bn_stats + moco_bn_fwd_train_given at batch 256, on an H100 SXM at a 700 W power limit
+# (tools/conv1x1_apply_times.py, results/conv1x1_apply_times_h100.json): 1.06-1.37x.  key: the forward without a
+# backward (the key encoder), where conv3's output is never written; otherwise the query encoder's, where the
+# statistics pass still writes it for bn3's backward.  shortcut: a downsample block (the shortcut BN in the apply).
+# Stage 3's downsample block in the query encoder measured 0.98x and keeps the apply pass.
+_APPLY_WINS = frozenset({(64, 256, False, False), (128, 512, False, False), (256, 1024, False, False),
+                         (64, 256, False, True), (128, 512, False, True),
+                         (64, 256, True, False), (128, 512, True, False), (256, 1024, True, False),
+                         (64, 256, True, True), (128, 512, True, True), (256, 1024, True, True)})
+
+
+def _apply_wins(M, Cin, Cout, key, shortcut):
+    return M >= 50176 and (Cin, Cout, key, shortcut) in _APPLY_WINS
+
+
+def conv1x1_bn_add_relu(conv, bn, x, residual, shortcut_bn=None, sc_stats=None, avgpool=False):
+    """``bn(conv(x), residual, shortcut_bn=shortcut_bn, avgpool=avgpool, ...)``: a bottleneck's conv3 -> bn3, with
+    ``sc_stats`` the shortcut BN's statistics from :func:`conv1x1_stats` (None where it did not take the shortcut).
+    Where :func:`conv1x1_stats` takes conv and the shape is in _APPLY_WINS, bn3 is applied by
+    moco_conv1x1_bn_add_relu_fwd, which recomputes conv(x) rather than reading it back.  With a backward to follow
+    (the query encoder) conv1x1_stats still writes conv(x), which bn3's backward reads; without one (the key encoder)
+    the statistics pass runs inside the same call without a store, and conv(x) is never allocated.  Same values,
+    running statistics and launch count as the path it replaces."""
+    if not avgpool and bn.relu and residual is not None and _conv1x1_ok(conv, bn, x, residual, shortcut_bn):
+        params = (x, residual, conv.weight, bn.weight, bn.bias) + (
+            (shortcut_bn.weight, shortcut_bn.bias) if shortcut_bn is not None else ())
+        key = not (torch.is_grad_enabled() and any(t.requires_grad for t in params))
+        N, Cin, H, W = x.shape
+        if _apply_wins(N * H * W, Cin, conv.weight.shape[0], key, shortcut_bn is not None):
+            w = conv.weight.to(torch.bfloat16).contiguous()
+            if key:
+                return _conv_bn_add_relu_nograd(x, w, bn, residual, shortcut_bn, sc_stats)
+            h, mean, invstd = _Conv1x1StatsFn.apply(x, w, bn._stats(), None)
+            return bn._add_relu(h, residual, shortcut_bn, (mean, invstd), sc_stats, recompute=(x, w))
+    h, st = conv1x1_stats(conv, bn, x, residual, shortcut_bn)
+    return bn(h, residual, shortcut_bn=shortcut_bn, avgpool=avgpool, stats=st, sc_stats=sc_stats)
+
+
+def _conv_bn_add_relu_nograd(x, w, bn, residual, shortcut_bn, sc_stats):
+    """relu(bn(conv2d(x, w)) + r) for a forward without a backward: one moco_conv1x1_bn_add_relu_fwd call runs the
+    statistics pass (no store) and the recomputing apply pass, plus the shortcut BN's statistics unless given."""
+    lib = _lib.load()
+    N, Cin, H, W = x.shape
+    C, M = w.shape[0], N * H * W
+    y = torch.empty((N, C, H, W), dtype=torch.bfloat16, device=x.device, memory_format=torch.channels_last)
+    f32 = lambda: torch.empty(C, dtype=torch.float32, device=x.device)
+    mean, invstd = f32(), f32()                     # kept alive until the call: the layer holds raw pointers
+    layer = _layer(bn.weight, bn.bias, mean, invstd, bn._stats())
+    sc, flags = None, 0
+    if shortcut_bn is not None:
+        sc_mean, sc_invstd = sc_stats if sc_stats is not None else (f32(), f32())
+        sc = _layer(shortcut_bn.weight, shortcut_bn.bias, sc_mean, sc_invstd, shortcut_bn._stats())
+        flags = _lib.BN_SC_STATS_GIVEN if sc_stats is not None else 0
+    ws = _workspace(x.device)
+    # algorithmic bytes: both passes read x; the apply reads the residual (+ the shortcut input for its statistics)
+    # and writes y
+    nbytes = M * 2 * (2 * Cin + C * (2 + (sc is not None and sc_stats is None)))
+    code = _timed("bn_fwd", nbytes, lambda: lib.moco_conv1x1_bn_add_relu_fwd(
+        x.data_ptr(), w.data_ptr(), residual.data_ptr(), y.data_ptr(), None, M, Cin, C, layer, sc, flags,
+        ws.data_ptr(), ws.numel(), _lib.cur_stream()))
+    _lib.check(code, "moco_conv1x1_bn_add_relu_fwd")
+    return y
+
+
 class BatchNormAct2d(nn.BatchNorm2d):
     """``nn.BatchNorm2d`` + optional residual add + optional ReLU (``forward(x, residual=None)``)."""
 
@@ -606,13 +682,13 @@ class BatchNormAct2d(nn.BatchNorm2d):
             return _BatchNormReluMaxPoolFn.apply(x, self.weight, self.bias, self._stats())
         return pool(self(x))
 
-    def _add_relu(self, x, residual, sc, stats=None, sc_stats=None):
+    def _add_relu(self, x, residual, sc, stats=None, sc_stats=None, recompute=None):
         params = (x, residual, self.weight, self.bias) + ((sc.weight, sc.bias) if sc is not None else ())
         want_mask = torch.is_grad_enabled() and any(t.requires_grad for t in params)
         return _BatchNormAddReluFn.apply(x, residual, self.weight, self.bias,
                                          sc.weight if sc is not None else None, sc.bias if sc is not None else None,
                                          self._stats(), sc._stats() if sc is not None else None, want_mask,
-                                         stats, sc_stats)
+                                         stats, sc_stats, recompute)
 
     def extra_repr(self):
         return super().extra_repr() + f", relu={self.relu}"

@@ -138,16 +138,6 @@ struct BnApplyArgs {
     const float* beta2;
 };
 
-// 8 mask bits of one vector of y, from the bf16 values as stored (a positive value that rounds to zero is off)
-__device__ __forceinline__ unsigned int relu_bits(const uint4& y) {
-    float r[8];
-    unpack8(y, r);
-    unsigned int b = 0u;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) b |= (r[k] > 0.f ? 1u : 0u) << k;
-    return b;
-}
-
 template <int kUnroll, int kCtas, bool kShortcut>
 __global__ void __launch_bounds__(kBnThreads, kCtas)
 bn_apply_kernel(const BnApplyArgs a) {
@@ -631,6 +621,12 @@ static cudaError_t stats_pass(const void* x, long long M, int C, float* running_
     s.mean = save_mean; s.invstd = save_invstd;
     s.running_mean = running_mean; s.running_var = running_var; s.num_batches_tracked = nbt;
     return run_stats<kBnStatsUnroll, kBnStatsCtas>(s, stream);
+}
+
+cudaError_t launch_bn_stats(const void* x, long long M, int C, const BnLayer& bn, void* ws, cudaStream_t stream) {
+    if (!bn_shape_ok(M, C)) return cudaErrorNotSupported;
+    return stats_pass(x, M, C, bn.running_mean, bn.running_var, bn.num_batches_tracked, bn.momentum, bn.eps,
+                      bn.save_mean, bn.save_invstd, ws, stream);
 }
 
 cudaError_t launch_bn_fwd_train(const void* x, const void* res, void* y, long long M, int C, const float* gamma,

@@ -31,6 +31,16 @@ __device__ __forceinline__ void unpack8(const uint4& u, float* f) {
     }
 }
 
+// 8 mask bits of one vector of y, from the bf16 values as stored (a positive value that rounds to zero is off)
+__device__ __forceinline__ unsigned int relu_bits(const uint4& y) {
+    float r[8];
+    unpack8(y, r);
+    unsigned int b = 0u;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) b |= (r[k] > 0.f ? 1u : 0u) << k;
+    return b;
+}
+
 // Sum the 8 * S per-thread accumulators (S per-channel sums of 8 channels) over the CTA's 32 row groups.  Returns, in
 // threads j < 64 * S, element j of the CTA partial: j = v * 8S + k with v = 16-byte lane (8 channels), k < 8 the first
 // sum, 8 <= k < 16 the second, 16 <= k < 24 the third.  Each element is added in the same order whatever S is.

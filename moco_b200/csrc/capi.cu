@@ -666,6 +666,37 @@ int moco_conv1x1_bn_stats(const void* x, const void* w, void* y, long long M, in
     return MOCO_OK;
 }
 
+int moco_conv1x1_bn_add_relu_fwd(const void* x, const void* w, const void* residual, void* y, void* mask, long long M,
+                                 int Cin, int Cout, const moco_bn_layer* bn, const moco_bn_layer* shortcut,
+                                 int stats_given, void* workspace, size_t workspace_bytes, void* stream_) {
+    g_err[0] = 0;
+    const bool passes = !(stats_given & MOCO_BN_STATS_GIVEN) || (shortcut && !(stats_given & MOCO_BN_SC_STATS_GIVEN));
+    if (!x || !w || !residual || !y || !bn_layer_fwd_ok(bn) || (shortcut && !bn_layer_fwd_ok(shortcut)) ||
+        (stats_given & ~(MOCO_BN_STATS_GIVEN | MOCO_BN_SC_STATS_GIVEN)) || (passes && !workspace) || misaligned16(x) ||
+        misaligned16(w) || misaligned16(residual) || misaligned16(y) || misaligned16(workspace) || y == x || y == w ||
+        y == residual || (mask && (mask == x || mask == y || mask == residual))) {
+        set_error("moco_conv1x1_bn_add_relu_fwd: bad argument (null / misaligned pointer, in-place, eps <= 0, one of "
+                  "running_mean / running_var, unknown stats_given bits; a statistics pass needs the workspace)");
+        return MOCO_ERR_INVALID;
+    }
+    if (M < 1 || M > 0x7fffff80LL || Cin < 64 || Cin % 64 != 0 || Cin > 65536 || Cout < 64 || Cout > 2048 ||
+        (Cout & (Cout - 1)) != 0) {
+        set_error("moco_conv1x1_bn_add_relu_fwd: needs 1 <= M < 2^31 - 128, Cin a multiple of 64 in [64, 65536] and "
+                  "Cout a power of two in [64, 2048] (M=%lld Cin=%d Cout=%d)", M, Cin, Cout);
+        return MOCO_ERR_UNSUPPORTED;
+    }
+    const size_t need = conv1x1_workspace_bytes() > bn_workspace_bytes() ? conv1x1_workspace_bytes()
+                                                                          : bn_workspace_bytes();
+    if (passes && workspace_bytes < need) {
+        set_error("moco_conv1x1_bn_add_relu_fwd: workspace too small (%zu < %zu)", workspace_bytes, need);
+        return MOCO_ERR_WORKSPACE;
+    }
+    cudaError_t e = launch_conv1x1_bn_add_relu(x, w, residual, y, mask, M, Cin, Cout, *bn, shortcut, stats_given,
+                                               workspace, static_cast<cudaStream_t>(stream_));
+    if (e != cudaSuccess) return cuda_fail("moco_conv1x1_bn_add_relu_fwd", e);
+    return MOCO_OK;
+}
+
 int moco_conv1x1_dgrad_bn_bwd(const void* dh, const void* w, void* g, long long M, int Cin, int Cout, const void* x,
                               const void* mask, const void* dy2, const void* x2, const moco_bn_layer* bn,
                               const moco_bn_layer* shortcut, void* workspace, size_t workspace_bytes, void* stream_) {

@@ -157,9 +157,16 @@ void bn_bwd_reduce_plan(long long M, int C, long long* passes, long long* ppc, i
 // sc's): dx (and the shortcut BN's input gradient dx2)
 cudaError_t launch_bn_bwd_apply_given(const void* g, const void* x, const void* x2, long long M, int C, const BnLayer& bn,
                                       const BnLayer* sc, void* dx, void* dx2, cudaStream_t stream);
+// the statistics pass alone (bn_stats_kernel): bn's save_mean / save_invstd and running statistics
+cudaError_t launch_bn_stats(const void* x, long long M, int C, const BnLayer& bn, void* ws, cudaStream_t stream);
 size_t conv1x1_workspace_bytes();
 cudaError_t launch_conv1x1_bn_stats(const void* x, const void* w, void* y, long long M, int Cin, int Cout,
                                     const BnLayer& bn, void* ws, cudaStream_t stream);
+// y = relu(bn(x . w^T) + r) recomputing the convolution (moco_conv1x1_bn_add_relu_fwd); given as for
+// launch_bn_fwd_given
+cudaError_t launch_conv1x1_bn_add_relu(const void* x, const void* w, const void* res, void* y, void* mask, long long M,
+                                       int Cin, int Cout, const BnLayer& bn, const BnLayer* sc, int given, void* ws,
+                                       cudaStream_t stream);
 // dgrad of a 1x1 convolution, g = mask . bf16(bf16(dH . w) + dy2), and the backward sums of the BatchNorm that
 // produced the convolution's input (moco_conv1x1_dgrad_bn_bwd)
 cudaError_t launch_conv1x1_dgrad_bn_bwd(const void* dh, const void* w, void* g, long long M, int Cin, int Cout,

@@ -40,6 +40,7 @@ static_assert(kBnThreads == 256, "the consumer warpgroups are the statistics pas
 
 struct Conv1x1Args {
     int M, Cin, m_tiles, ppc, R, stages;   // ppc = tiles per CTA; R = CTAs per column slice
+    int store;                             // 0: the statistics only, y is not written
     float momentum, eps;
     float* partial;                        // [slabs][R][128], bn_stats_kernel's layout
     unsigned int* counters;                // [slabs]
@@ -65,6 +66,46 @@ struct Conv1x1Shape {
 struct ConsumerSync {
     __device__ __forceinline__ void operator()() const { named_bar_sync(3, kBnThreads); }
 };
+
+// The mainloop of the forward kernels, one 128-row tile of column slice nb.  Producer: the Cin / 64 chunks of the x
+// slab and the w slab into the ring.  Consumers: wgmma over them in increasing K, so every kernel that runs it computes
+// the same accumulator for the same tile.  (st, ph): the ring position, carried from tile to tile.
+template <int BN>
+__device__ __forceinline__ void conv1x1_load_tile(const CUtensorMap* tm_x, const CUtensorMap* tm_w, uint8_t* ring,
+                                                  uint64_t* full, uint64_t* empty, int NS, int& st, uint32_t& ph,
+                                                  int tile, int nb, int ksteps) {
+    using S = Conv1x1Shape<BN>;
+    for (int kc = 0; kc < ksteps; ++kc) {
+        mbar_wait(&empty[st], ph ^ 1u);
+        mbar_arrive_expect_tx(&full[st], (uint32_t)S::kStage);   // OOB rows count too (zero-filled)
+        uint8_t* s = ring + (size_t)st * S::kStage;
+        tma_load_2d(tm_x, &full[st], s, kc * 64, tile * kCvBM);
+        tma_load_2d(tm_w, &full[st], s + S::kA, kc * 64, nb * BN);
+        if (++st == NS) { st = 0; ph ^= 1u; }
+    }
+}
+
+template <int BN>
+__device__ __forceinline__ void conv1x1_mma_tile(float (&acc)[BN / 2], uint64_t a_desc0, uint64_t b_desc0, uint64_t* full,
+                                                 uint64_t* empty, int NS, int& st, uint32_t& ph, int ksteps, int t) {
+    constexpr uint64_t kStageUnits = Conv1x1Shape<BN>::kStage >> 4;
+    int prev = 0;
+    for (int kc = 0; kc < ksteps; ++kc) {
+        mbar_wait(&full[st], ph);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+            wgmma_ss<BN>(acc, a_desc0 + st * kStageUnits + 2 * k, b_desc0 + st * kStageUnits + 2 * k, (kc | k) != 0);
+        wgmma_commit();
+        wgmma_wait<1>();                                          // the previous chunk's wgmmas have completed
+        if (kc > 0 && t == 0) mbar_arrive(&empty[prev]);
+        prev = st;
+        if (++st == NS) { st = 0; ph ^= 1u; }
+    }
+    wgmma_wait<0>();
+    reg_fence(acc);
+    if (t == 0) mbar_arrive(&empty[prev]);
+}
 
 template <int BN>
 __global__ void __launch_bounds__(kCvThreads, 1)
@@ -106,17 +147,8 @@ conv1x1_stats_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_cons
             // ---------------------------------------------------- TMA producer
             int st = 0;
             uint32_t ph = 0;
-            for (int it = first; it < t1 - t0; ++it) {
-                const int tile = it < 0 ? 0 : t0 + it;
-                for (int kc = 0; kc < ksteps; ++kc) {
-                    mbar_wait(&empty[st], ph ^ 1u);
-                    mbar_arrive_expect_tx(&full[st], (uint32_t)S::kStage);   // OOB rows count too (zero-filled)
-                    uint8_t* s = ring + (size_t)st * S::kStage;
-                    tma_load_2d(&tm_x, &full[st], s, kc * 64, tile * kCvBM);
-                    tma_load_2d(&tm_w, &full[st], s + S::kA, kc * 64, nb * BN);
-                    if (++st == NS) { st = 0; ph ^= 1u; }
-                }
-            }
+            for (int it = first; it < t1 - t0; ++it)
+                conv1x1_load_tile<BN>(&tm_x, &tm_w, ring, full, empty, NS, st, ph, it < 0 ? 0 : t0 + it, nb, ksteps);
         }
         return;
     }
@@ -128,7 +160,6 @@ conv1x1_stats_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_cons
     const int v = threadIdx.x & (kBnLanes - 1), rl = threadIdx.x >> 3;   // bn_stats_kernel's thread layout
     const uint64_t a_desc0 = make_sw128_desc(smem_u32(ring + wg * 64 * 128), 16, 1024);
     const uint64_t b_desc0 = make_sw128_desc(smem_u32(ring + S::kA), 16, 1024);
-    constexpr uint64_t kStageUnits = S::kStage >> 4;
     float acc[BN / 2];
     float sacc[kSlabs][16];                                       // per slab: 8 sums of (y - h), 8 of (y - h)^2
     float sh[kSlabs][8];
@@ -140,23 +171,7 @@ conv1x1_stats_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_cons
     uint32_t ph = 0;
     for (int it = first; it < t1 - t0; ++it) {
         const int tile = it < 0 ? 0 : t0 + it;
-        int prev = 0;
-        for (int kc = 0; kc < ksteps; ++kc) {
-            mbar_wait(&full[st], ph);
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-                wgmma_ss<BN>(acc, a_desc0 + st * kStageUnits + 2 * k, b_desc0 + st * kStageUnits + 2 * k,
-                             (kc | k) != 0);
-            wgmma_commit();
-            wgmma_wait<1>();                                      // the previous chunk's wgmmas have completed
-            if (kc > 0 && t == 0) mbar_arrive(&empty[prev]);
-            prev = st;
-            if (++st == NS) { st = 0; ph ^= 1u; }
-        }
-        wgmma_wait<0>();
-        reg_fence(acc);
-        if (t == 0) mbar_arrive(&empty[prev]);
+        conv1x1_mma_tile<BN>(acc, a_desc0, b_desc0, full, empty, NS, st, ph, ksteps, t);
 
         if (it == first) {                                        // tile 0: the shift y[0, c], as rounded
             if (wg == 0 && warp == 0 && lane < 4) {
@@ -191,7 +206,7 @@ conv1x1_stats_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_cons
         }
         fence_proxy_async();                                      // generic smem writes -> visible to the TMA store
         named_bar_sync(3, kBnThreads);                            // both halves staged (and the buffer's last readers done)
-        if (t == 0) {
+        if (t == 0 && a.store) {
 #pragma unroll
             for (int sl = 0; sl < BN / 64; ++sl)
                 tma_store_2d(&tm_y, ob + sl * 8192, nb * BN + sl * 64, tile * kCvBM + wg * 64);
@@ -258,9 +273,12 @@ static cudaError_t launch_bn(const void* x, const void* w, void* y, int M, int C
     a.partial = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 256);
     a.mean = bn.save_mean; a.invstd = bn.save_invstd;
     a.running_mean = bn.running_mean; a.running_var = bn.running_var; a.num_batches_tracked = bn.num_batches_tracked;
+    a.store = y != nullptr;
     CUtensorMap tm_x, tm_w, tm_y;
-    if (!make_tmap(&tm_x, x, M, Cin, kCvBM) || !make_tmap(&tm_w, w, Cout, Cin, BN) || !make_tmap(&tm_y, y, M, Cout, 64))
+    if (!make_tmap(&tm_x, x, M, Cin, kCvBM) || !make_tmap(&tm_w, w, Cout, Cin, BN))
         return cudaErrorUnknown;
+    if (y == nullptr) tm_y = tm_x;                         // not used
+    else if (!make_tmap(&tm_y, y, M, Cout, 64)) return cudaErrorUnknown;
     {
         std::lock_guard<std::mutex> lock(g_kernel_cache_mutex);
         KernelCache& kc = kernel_cache(BN / 64 - 1);
@@ -282,6 +300,235 @@ cudaError_t launch_conv1x1_bn_stats(const void* x, const void* w, void* y, long 
         return cudaErrorNotSupported;
     if (Cout % 128 == 0) return launch_bn<128>(x, w, y, (int)M, Cin, Cout, bn, ws, stream);
     return launch_bn<64>(x, w, y, (int)M, Cin, Cout, bn, ws, stream);
+}
+
+// ---- the residual BatchNorm applied in a second pass of the GEMM ----------------------------------------------------
+// Once the statistics of h = x . w^T are known (the pass above), the block output y = relu(bn(h) + r) is computed from
+// x again rather than from h read back: for conv3 of a bottleneck (K = Cin = Cout / 4) the GEMM costs less than the
+// 8 bytes per element of h written and read.  The mainloop is conv1x1_load_tile / conv1x1_mma_tile with the same BN,
+// so the accumulator of a tile is the one the statistics pass rounded and stored.  The epilogue is bn_apply_kernel's
+// arithmetic (bn_nhwc.cu): h rounded to bf16, z = fmaf(h, ca, cb) + r with ca = gamma * invstd, cb = fmaf(-mean, ca,
+// beta), ReLU, one rounding; with a shortcut BN r = bf16(fmaf(s, ca2, cb2) + 0) of the shortcut convolution's raw
+// output s.  The mask bytes (nullable) are relu_bits of the staged output.
+// The TMA producer loads the r (or s) tile into two buffers, one tile ahead of the consumers; y is staged in place over
+// it and stored from there.  The grid is one wave: a column slice per blockIdx.x, contiguous tile ranges per blockIdx.y.
+struct Conv1x1ApplyArgs {
+    int M, Cin, C, m_tiles, ppc, stages;   // C = Cout; ppc = tiles per CTA
+    const float* mean;
+    const float* invstd;
+    const float* gamma;
+    const float* beta;
+    const float* mean2;                    // kShortcut: the shortcut BN
+    const float* invstd2;
+    const float* gamma2;
+    const float* beta2;
+    uint8_t* mask;                         // nullable: uint8 [M, C / 8]
+};
+
+template <int BN>
+struct Conv1x1ApplyShape {
+    static constexpr int kTile = (BN / 64) * kSlab;        // r / y tile: [BN / 64 column slabs][128 rows x 64 bf16]
+    static constexpr int kFixed = 2 * kTile + 4 * BN * 4;  // two tile buffers, ca / cb / ca2 / cb2
+};
+
+template <int BN, bool kShortcut>
+__global__ void __launch_bounds__(kCvThreads, 1)
+conv1x1_bn_apply_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w,
+                        const __grid_constant__ CUtensorMap tm_r, const __grid_constant__ CUtensorMap tm_y,
+                        const Conv1x1ApplyArgs a) {
+    using S = Conv1x1Shape<BN>;
+    using E = Conv1x1ApplyShape<BN>;
+    constexpr int kSlabs = BN / 64;
+    extern __shared__ __align__(1024) uint8_t smem[];
+    if ((smem_u32(smem) & 1023u) != 0u) __trap();
+    const int NS = a.stages;
+    uint8_t* ring = smem;                                          // NS x (x slab, w slab)
+    uint8_t* epi = ring + (size_t)NS * S::kStage;                  // [2] r tiles, then y
+    float* ca = reinterpret_cast<float*>(epi + 2 * E::kTile);      // [BN] each
+    float* cb = ca + BN;
+    float* ca2 = cb + BN;
+    float* cb2 = ca2 + BN;
+    uint64_t* full = reinterpret_cast<uint64_t*>(cb2 + BN);
+    uint64_t* empty = full + NS;
+    uint64_t* efull = empty + NS;
+    uint64_t* eempty = efull + 2;
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int nb = blockIdx.x;
+    const int t0 = blockIdx.y * a.ppc;
+    const int t1 = min(t0 + a.ppc, a.m_tiles);
+    const int ksteps = a.Cin >> 6;
+
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&tm_x);
+        tma_prefetch_desc(&tm_w);
+        tma_prefetch_desc(&tm_r);
+        tma_prefetch_desc(&tm_y);
+        for (int s = 0; s < NS; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
+        for (int b = 0; b < 2; ++b) { mbar_init(&efull[b], 1); mbar_init(&eempty[b], kBnThreads); }
+        fence_mbar_init();
+    }
+    if (threadIdx.x < BN) {                                        // bn_apply_kernel's coefficients
+        const int c = nb * BN + threadIdx.x;
+        const float k = __ldg(a.gamma + c) * __ldg(a.invstd + c);
+        ca[threadIdx.x] = k;
+        cb[threadIdx.x] = fmaf(-__ldg(a.mean + c), k, __ldg(a.beta + c));
+        if constexpr (kShortcut) {
+            const float k2 = __ldg(a.gamma2 + c) * __ldg(a.invstd2 + c);
+            ca2[threadIdx.x] = k2;
+            cb2[threadIdx.x] = fmaf(-__ldg(a.mean2 + c), k2, __ldg(a.beta2 + c));
+        }
+    }
+    __syncthreads();
+
+    if (warp >= 8) {
+        setmaxnreg_dec<40>();
+        if (warp == 8 && elect_one()) {
+            // ---------------------------------------------------- TMA producer
+            int st = 0;
+            uint32_t ph = 0;
+            for (int it = 0; it < t1 - t0; ++it) {
+                const int tile = t0 + it, eb = it & 1;
+                mbar_wait(&eempty[eb], ((it >> 1) & 1) ^ 1u);
+                mbar_arrive_expect_tx(&efull[eb], (uint32_t)E::kTile);   // OOB rows count too (zero-filled)
+#pragma unroll
+                for (int s = 0; s < kSlabs; ++s)
+                    tma_load_2d(&tm_r, &efull[eb], epi + eb * E::kTile + s * kSlab, nb * BN + s * 64, tile * kCvBM);
+                conv1x1_load_tile<BN>(&tm_x, &tm_w, ring, full, empty, NS, st, ph, tile, nb, ksteps);
+            }
+        }
+        return;
+    }
+    // ------------------------------------------------------------ consumer warpgroups
+    setmaxnreg_inc<232>();
+    const int wg = warp >> 2, t = threadIdx.x & 127;
+    const int rloc = wg * 64 + (warp & 3) * 16 + (lane >> 2);    // tile rows rloc and rloc + 8
+    const int ccol = 2 * (lane & 3);                              // first of this thread's two columns per 8
+    const int v = threadIdx.x & (kBnLanes - 1), rl = threadIdx.x >> 3;   // 8-channel vector, row of the mask pass
+    const uint64_t a_desc0 = make_sw128_desc(smem_u32(ring + wg * 64 * 128), 16, 1024);
+    const uint64_t b_desc0 = make_sw128_desc(smem_u32(ring + S::kA), 16, 1024);
+    const int mask_row = a.C >> 3;
+    float acc[BN / 2];
+    int st = 0;
+    uint32_t ph = 0;
+    for (int it = 0; it < t1 - t0; ++it) {
+        const int tile = t0 + it, eb = it & 1;
+        conv1x1_mma_tile<BN>(acc, a_desc0, b_desc0, full, empty, NS, st, ph, ksteps, t);
+
+        // ---- epilogue: y = relu(fmaf(bf16(acc), ca, cb) + r), in place over r -> TMA store; mask bytes from the tile
+        uint8_t* e = epi + eb * E::kTile;
+        mbar_wait(&efull[eb], (it >> 1) & 1);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int row = rloc + 8 * h;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                __nv_bfloat162* p = reinterpret_cast<__nv_bfloat162*>(e + (j >> 3) * kSlab + row * 128 +
+                                                                      (((j & 7) ^ (row & 7)) << 4) + (lane & 3) * 4);
+                const float2 r2 = __bfloat1622float2(*p);
+                float z[2];
+#pragma unroll
+                for (int q = 0; q < 2; ++q) {
+                    const int c = 8 * j + ccol + q;
+                    float r = q ? r2.y : r2.x;
+                    if constexpr (kShortcut)
+                        r = __bfloat162float(__float2bfloat16_rn(__fadd_rn(fmaf(r, ca2[c], cb2[c]), 0.f)));
+                    const float hv = __bfloat162float(__float2bfloat16_rn(acc[4 * j + 2 * h + q]));
+                    z[q] = fmaxf(__fadd_rn(fmaf(hv, ca[c], cb[c]), r), 0.f);
+                }
+                *p = __floats2bfloat162_rn(z[0], z[1]);
+            }
+        }
+        fence_proxy_async();                                      // generic smem writes -> visible to the TMA store
+        named_bar_sync(3, kBnThreads);                            // the whole tile staged
+        if (threadIdx.x == 0) {
+#pragma unroll
+            for (int s = 0; s < kSlabs; ++s) tma_store_2d(&tm_y, e + s * kSlab, nb * BN + s * 64, tile * kCvBM);
+            bulk_commit();
+        }
+        if (a.mask != nullptr) {
+#pragma unroll
+            for (int p = 0; p < kCvBM / kBnRows; ++p) {
+                const int row = p * kBnRows + rl;
+                const long long grow = (long long)tile * kCvBM + row;
+                if (grow < a.M) {
+#pragma unroll
+                    for (int s = 0; s < kSlabs; ++s) {
+                        const uint4 u = *reinterpret_cast<const uint4*>(e + s * kSlab + row * 128 + ((v ^ (row & 7)) << 4));
+                        a.mask[grow * mask_row + nb * (BN / 8) + s * 8 + v] = (uint8_t)relu_bits(u);
+                    }
+                }
+            }
+        }
+        if (threadIdx.x == 0) bulk_wait_read<0>();               // the store has read y out of the buffer
+        mbar_arrive(&eempty[eb]);
+    }
+    if (threadIdx.x == 0) bulk_wait<0>();
+}
+
+template <int BN, bool SC>
+static cudaError_t launch_apply(const void* x, const void* w, const void* res, void* y, void* mask, int M, int Cin,
+                                int Cout, const BnLayer& bn, const BnLayer* sc, cudaStream_t stream) {
+    using S = Conv1x1Shape<BN>;
+    using E = Conv1x1ApplyShape<BN>;
+    Conv1x1ApplyArgs a{};
+    a.M = M; a.Cin = Cin; a.C = Cout;
+    a.m_tiles = (M + kCvBM - 1) / kCvBM;
+    int dev = 0, sms = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (e != cudaSuccess) return e;
+    const int slices = Cout / BN;
+    int R = sms / slices;                                  // one CTA per SM
+    if (R < 1) R = 1;
+    a.ppc = (a.m_tiles + R - 1) / R;
+    R = (a.m_tiles + a.ppc - 1) / a.ppc;
+    constexpr int kBarBytes = 256;
+    int stages = (kSmemBudget - E::kFixed - kBarBytes) / S::kStage;
+    if (stages > 8) stages = 8;
+    if (stages < 2) return cudaErrorNotSupported;
+    a.stages = stages;
+    const int smem = stages * S::kStage + E::kFixed + kBarBytes;
+    a.mean = bn.save_mean; a.invstd = bn.save_invstd; a.gamma = bn.gamma; a.beta = bn.beta;
+    if (SC) { a.mean2 = sc->save_mean; a.invstd2 = sc->save_invstd; a.gamma2 = sc->gamma; a.beta2 = sc->beta; }
+    a.mask = static_cast<uint8_t*>(mask);
+    CUtensorMap tm_x, tm_w, tm_r, tm_y;
+    if (!make_tmap(&tm_x, x, M, Cin, kCvBM) || !make_tmap(&tm_w, w, Cout, Cin, BN) ||
+        !make_tmap(&tm_r, res, M, Cout, kCvBM) || !make_tmap(&tm_y, y, M, Cout, kCvBM))
+        return cudaErrorUnknown;
+    {
+        std::lock_guard<std::mutex> lock(g_kernel_cache_mutex);
+        KernelCache& kc = kernel_cache(3 + 2 * (BN / 64 - 1) + (SC ? 1 : 0));
+        if (kc.smem_set < smem) {
+            e = cudaFuncSetAttribute(conv1x1_bn_apply_kernel<BN, SC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+            if (e != cudaSuccess) return e;
+            kc.smem_set = smem;
+        }
+    }
+    conv1x1_bn_apply_kernel<BN, SC><<<dim3(slices, R), kCvThreads, smem, stream>>>(tm_x, tm_w, tm_r, tm_y, a);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_conv1x1_bn_add_relu(const void* x, const void* w, const void* res, void* y, void* mask, long long M,
+                                       int Cin, int Cout, const BnLayer& bn, const BnLayer* sc, int given, void* ws,
+                                       cudaStream_t stream) {
+    // Cout is the BatchNorm's C (a power of two in [64, 2048]), as in the statistics and apply passes it replaces
+    if (M < 1 || M > 0x7fffff80LL || Cin < 64 || Cin % 64 != 0 || Cin > 65536 || Cout < 64 || Cout > 2048 ||
+        (Cout & (Cout - 1)) != 0)
+        return cudaErrorNotSupported;
+    const int BN = Cout % 128 == 0 ? 128 : 64;
+    cudaError_t e = cudaSuccess;
+    if (!(given & MOCO_BN_STATS_GIVEN))                    // the statistics pass without storing h
+        e = BN == 128 ? launch_bn<128>(x, w, nullptr, (int)M, Cin, Cout, bn, ws, stream)
+                      : launch_bn<64>(x, w, nullptr, (int)M, Cin, Cout, bn, ws, stream);
+    if (e == cudaSuccess && sc != nullptr && !(given & MOCO_BN_SC_STATS_GIVEN))
+        e = launch_bn_stats(res, M, Cout, *sc, ws, stream);
+    if (e != cudaSuccess) return e;
+    if (BN == 128)
+        return sc != nullptr ? launch_apply<128, true>(x, w, res, y, mask, (int)M, Cin, Cout, bn, sc, stream)
+                             : launch_apply<128, false>(x, w, res, y, mask, (int)M, Cin, Cout, bn, sc, stream);
+    return sc != nullptr ? launch_apply<64, true>(x, w, res, y, mask, (int)M, Cin, Cout, bn, sc, stream)
+                         : launch_apply<64, false>(x, w, res, y, mask, (int)M, Cin, Cout, bn, sc, stream);
 }
 
 // ---- backward: the input gradient with the producing BatchNorm's backward reduction ---------------------------------

@@ -66,11 +66,9 @@ class _Bottleneck(nn.Module):
         y = self.bn2(self.conv2(y))
         r = bn_mod.hand_over(x)                   # x's second consumer: its gradient is summed in x's producer
         if self.short is None:
-            h, st = bn_mod.conv1x1_stats(self.conv3, self.bn3, y, r)
-            return self.bn3(h, r, avgpool=avgpool, stats=st)
+            return bn_mod.conv1x1_bn_add_relu(self.conv3, self.bn3, y, r, avgpool=avgpool)
         s, sc_st = bn_mod.conv1x1_stats(self.short[0], self.short[1], r)
-        h, st = bn_mod.conv1x1_stats(self.conv3, self.bn3, y, s, self.short[1])
-        return self.bn3(h, s, shortcut_bn=self.short[1], avgpool=avgpool, stats=st, sc_stats=sc_st)   # one BN group
+        return bn_mod.conv1x1_bn_add_relu(self.conv3, self.bn3, y, s, self.short[1], sc_st, avgpool)   # one BN group
 
 
 class StemConv(nn.Conv2d):

@@ -21,6 +21,8 @@ if ROOT not in sys.path:
 
 # (class, substrings of the kernel name); the first class with a matching substring wins
 CLASSES = [
+    # conv3 recomputed with bn3's apply in its epilogue; first, since its name contains "bn_apply_kernel"
+    ("conv1x1_bn_apply", ("conv1x1_bn_apply_kernel",)),
     ("conv1x1_stats", ("conv1x1_stats_kernel",)),     # csrc/conv1x1_sm90.cu: 1x1 forward + the next BN's statistics
     # 1x1 dgrad + the producing BN's backward sums; before conv_dgrad, which takes any name containing "dgrad"
     ("conv1x1_dgrad_bn", ("conv1x1_dgrad_bn_bwd_kernel",)),
