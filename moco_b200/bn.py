@@ -4,9 +4,10 @@ The reference's encoders apply ``nn.BatchNorm2d`` -> [``out += residual``] -> [`
 ``moco/models/resnet.py:42-63,74-102,114,139-143,156-157``; ShuffleBN (``moco/util.py:69-93``) exists for exactly these
 batch statistics, and left to ATen's channels_last kernels they take most of the GPU time of a step.  :class:`BatchNormAct2d` is an ``nn.BatchNorm2d`` (same parameters,
 buffers and ``state_dict`` keys, same running-statistics updates) whose training-mode forward / backward on CUDA
-bf16 channels_last activations are two launches each of ``csrc/bn_nhwc.cu`` (``moco_bn_fwd_train`` / ``moco_bn_bwd``).
-A block's residual BatchNorm, ``relu(bn(x) + r)``, runs ``moco_bn_add_relu_*`` instead: the forward writes the ReLU
-mask as bits for the backward rather than having it re-read ``y``, and in a downsample block (``forward(x, residual,
+bf16 channels_last activations are two launches each of ``csrc/bn_nhwc.cu``: ``moco_bn_fwd_train_given``
+(:func:`_bn_fwd`) and ``moco_bn_bwd`` (:func:`_bn_bwd`).
+A block's residual BatchNorm, ``relu(bn(x) + r)``, has the forward write the ReLU mask as bits and the backward read
+them (``moco_bn_add_relu_bwd``) rather than re-read ``y``, and in a downsample block (``forward(x, residual,
 shortcut_bn=...)``) the shortcut's BatchNorm runs inside the same passes, so neither its output nor the gradient
 between the two BatchNorms is ever written.  The stem's BatchNorm + ReLU and its max pool (``forward_maxpool``) run
 as ``moco_bn_relu_maxpool_fwd_train``: the pool applies the BatchNorm to each tap, so the stem's full-resolution
@@ -90,6 +91,102 @@ def _take_handed(ctx):
     return _grad_rows(g)
 
 
+def _ptr(t):
+    return t.data_ptr() if t is not None else None
+
+
+def _f32(C, device):
+    return torch.empty(C, dtype=torch.float32, device=device)
+
+
+def _layer(weight, bias, mean, invstd, stats=None, dgamma=None, dbeta=None):
+    """moco_bn_layer of one BatchNorm: stats = (running_mean, running_var, num_batches_tracked, momentum, eps)."""
+    rm, rv, nbt, momentum, eps = stats if stats is not None else (None, None, None, 0.0, 0.0)
+    return _lib.BnLayer(_ptr(weight), _ptr(bias), _ptr(rm), _ptr(rv), _ptr(nbt), float(momentum), float(eps),
+                        _ptr(mean), _ptr(invstd), _ptr(dgamma), _ptr(dbeta))
+
+
+def _bn_fwd(x, residual, y, mask, relu, bn, sc=None, given=None, sc_given=None, recompute=None):
+    """The training forward into ``y`` (and the ReLU mask bits into ``mask``): y = relu?(bn(x) [+ r]), r = residual
+    or, with ``sc``, bf16(sc(residual)).  bn / sc: (weight, bias, stats as for :func:`_layer`).  given / sc_given:
+    (mean, invstd) the producing convolution computed (:func:`conv1x1_stats`, which also updated the running
+    statistics); that layer's statistics pass is skipped.  recompute: (a, w) with x = conv2d(a, w) of a 1x1
+    convolution: moco_conv1x1_bn_add_relu_fwd computes y from a instead of reading x, which may then be None when
+    its statistics are not given either.  Returns (mean, invstd, sc_mean, sc_invstd)."""
+    lib = _lib.load()
+    N, C, H, W = y.shape
+    M = N * H * W
+    mean, invstd = given if given is not None else (_f32(C, y.device), _f32(C, y.device))
+    layer = _layer(bn[0], bn[1], mean, invstd, bn[2])
+    sc_layer, sc_mean, sc_invstd = None, None, None
+    if sc is not None:
+        sc_mean, sc_invstd = sc_given if sc_given is not None else (_f32(C, y.device), _f32(C, y.device))
+        sc_layer = _layer(sc[0], sc[1], sc_mean, sc_invstd, sc[2])
+    flags = (_lib.BN_STATS_GIVEN if given is not None else 0) | (_lib.BN_SC_STATS_GIVEN if sc_given is not None else 0)
+    ws = _workspace(y.device)
+    # algorithmic bytes: a statistics pass reads its layer's input; the apply pass reads x (+ residual) and writes y
+    # (+ mask bits).  recompute: both of bn's passes read a in place of x.
+    sc_pass = sc is not None and sc_given is None
+    mask_bytes = M * C // 8 if mask is not None else 0
+    if recompute is not None:
+        a, w = recompute
+        Cin = a.shape[1]
+        name = "moco_conv1x1_bn_add_relu_fwd"
+        nbytes = 2 * M * (Cin * (1 + (given is None)) + C * (2 + sc_pass)) + mask_bytes
+        args = (a.data_ptr(), w.data_ptr(), residual.data_ptr(), y.data_ptr(), _ptr(mask), M, Cin, C, layer, sc_layer,
+                flags, ws.data_ptr(), ws.numel())
+    else:
+        name = "moco_bn_fwd_train_given"
+        nbytes = 2 * M * C * (2 + (residual is not None) + (given is None) + sc_pass) + mask_bytes
+        args = (x.data_ptr(), _ptr(residual), y.data_ptr(), _ptr(mask), M, C, int(relu), layer, sc_layer, flags,
+                ws.data_ptr(), ws.numel())
+    _lib.check(_timed("bn_fwd", nbytes, lambda: getattr(lib, name)(*args, _lib.cur_stream())), name)
+    return mean, invstd, sc_mean, sc_invstd
+
+
+def _bn_bwd(dy, x, bn, relu, has_res=False, y=None, mask=None, dy2=None, sc=None, dres=None, sums=None):
+    """The training backward of :func:`_bn_fwd`.  bn: (weight, bias, mean, invstd); sc: (weight, mean, invstd, input)
+    of the shortcut BN.  The ReLU mask is ``mask``, the forward's bits, else taken from ``y`` (relu and has_res) or
+    recomputed from x (relu).  dy2: a second gradient of y, summed with dy inside both passes.  dres: where the
+    masked gradient -- with sc, the shortcut BN's input gradient -- is written.  sums: (dgamma, dbeta) of an
+    already masked dy (:func:`_dgrad_bn_bwd`): the element-wise pass alone.
+    Returns (dx, dgamma, dbeta, sc_dgamma, sc_dbeta)."""
+    lib = _lib.load()
+    N, C, H, W = x.shape
+    M = N * H * W
+    weight, bias, mean, invstd = bn
+    dx = torch.empty_like(x)
+    dgamma, dbeta = sums if sums is not None else (_f32(C, x.device), _f32(C, x.device))
+    layer = _layer(weight, bias, mean, invstd, dgamma=dgamma, dbeta=dbeta)
+    sc_layer, sc_dgamma, sc_dbeta, x2 = None, None, None, None
+    if sc is not None:
+        sc_weight, sc_mean, sc_invstd, x2 = sc
+        sc_dgamma, sc_dbeta = _f32(C, x.device), _f32(C, x.device)
+        sc_layer = _layer(sc_weight, None, sc_mean, sc_invstd, dgamma=sc_dgamma, dbeta=sc_dbeta)
+    ws = _workspace(x.device)
+    # algorithmic bytes: the reduce and the apply pass each read dy (+ dy2), x (+ y | mask bits) (+ the shortcut
+    # input); the apply pass writes dx (+ d residual)
+    passes = 1 if sums is not None else 2
+    reads = 2 + (y is not None) + (x2 is not None) + (dy2 is not None)
+    nbytes = 2 * M * C * (passes * reads + 1 + (dres is not None)) + (2 * (M * C // 8) if mask is not None else 0)
+    tail = (ws.data_ptr(), ws.numel())
+    if sums is not None:
+        name = "moco_bn_bwd_apply_given"
+        args = (dy.data_ptr(), x.data_ptr(), None, M, C, layer, None, dx.data_ptr(), None)
+    elif mask is None:
+        name = "moco_bn_bwd"
+        args = (dy.data_ptr(), x.data_ptr(), _ptr(y), M, C, weight.data_ptr(), bias.data_ptr(), mean.data_ptr(),
+                invstd.data_ptr(), int(relu), int(has_res), dx.data_ptr(), _ptr(dres), dgamma.data_ptr(),
+                dbeta.data_ptr()) + tail
+    else:
+        name = "moco_bn_add_relu_bwd" if dy2 is None else "moco_bn_add_relu_bwd2"
+        grads = (dy.data_ptr(),) if dy2 is None else (dy.data_ptr(), dy2.data_ptr())
+        args = grads + (x.data_ptr(), _ptr(x2), mask.data_ptr(), M, C, layer, sc_layer, dx.data_ptr(),
+                        _ptr(dres)) + tail
+    _lib.check(_timed("bn_bwd", nbytes, lambda: getattr(lib, name)(*args, _lib.cur_stream())), name)
+    return dx, dgamma, dbeta, sc_dgamma, sc_dbeta
+
+
 class _BatchNormActFn(torch.autograd.Function):
     """y = relu?(batch_norm_train(x) [+ residual]); x, residual, y bf16 channels_last; weight / bias fp32."""
 
@@ -98,30 +195,9 @@ class _BatchNormActFn(torch.autograd.Function):
                 given=None):
         """given: (mean, invstd) already computed by the producing convolution (:func:`conv1x1_stats`), which also
         updated the running statistics: only the apply pass runs."""
-        lib = _lib.load()
-        N, C, H, W = x.shape
-        M = N * H * W
         y = torch.empty_like(x)                                   # keeps the channels_last strides
-        ptr = lambda t: t.data_ptr() if t is not None else None
-        if given is not None:
-            mean, invstd = given
-            bn = _layer(weight, bias, mean, invstd, (running_mean, running_var, num_batches_tracked, momentum, eps))
-            # algorithmic bytes: apply reads x (+ residual) and writes y
-            code = _timed("bn_fwd", M * C * 2 * (2 + (residual is not None)), lambda: lib.moco_bn_fwd_train_given(
-                x.data_ptr(), ptr(residual), y.data_ptr(), None, M, C, int(relu), bn, None, _lib.BN_STATS_GIVEN,
-                None, 0, _lib.cur_stream()))
-            _lib.check(code, "moco_bn_fwd_train_given")
-        else:
-            mean = torch.empty(C, dtype=torch.float32, device=x.device)
-            invstd = torch.empty_like(mean)
-            ws = _workspace(x.device)
-            # algorithmic bytes: statistics read x; apply reads x (+ residual) and writes y
-            code = _timed("bn_fwd", M * C * 2 * (3 + (residual is not None)), lambda: lib.moco_bn_fwd_train(
-                x.data_ptr(), ptr(residual), y.data_ptr(), M, C, weight.data_ptr(), bias.data_ptr(),
-                ptr(running_mean), ptr(running_var), ptr(num_batches_tracked),
-                float(momentum), float(eps), int(relu), mean.data_ptr(), invstd.data_ptr(), ws.data_ptr(), ws.numel(),
-                _lib.cur_stream()))
-            _lib.check(code, "moco_bn_fwd_train")
+        stats = (running_mean, running_var, num_batches_tracked, momentum, eps)
+        mean, invstd, _, _ = _bn_fwd(x, residual, y, None, relu, (weight, bias, stats), given=given)
         ctx.relu = bool(relu)
         ctx.has_res = residual is not None
         # the ReLU mask of the backward is recomputed from x unless a residual went into it
@@ -131,40 +207,13 @@ class _BatchNormActFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         x, y, weight, bias, mean, invstd = ctx.saved_tensors
-        lib = _lib.load()
-        N, C, H, W = x.shape
-        if dy.dtype != torch.bfloat16:
-            dy = dy.to(torch.bfloat16)
-        dy = dy.contiguous(memory_format=torch.channels_last)
-        dx = torch.empty_like(x)
+        dy = _grad_rows(dy)
         want_res = ctx.has_res and ctx.needs_input_grad[3]
+        dres = torch.empty_like(x) if want_res and ctx.relu else None
+        dx, dgamma, dbeta, _, _ = _bn_bwd(dy, x, (weight, bias, mean, invstd), ctx.relu, ctx.has_res, y=y, dres=dres)
         if want_res and not ctx.relu:
-            dres, dres_ptr = dy, None                             # without a ReLU the residual's gradient is dy itself
-        elif want_res:
-            dres = torch.empty_like(x)
-            dres_ptr = dres.data_ptr()
-        else:
-            dres, dres_ptr = None, None
-        dgamma = torch.empty(C, dtype=torch.float32, device=x.device)
-        dbeta = torch.empty_like(dgamma)
-        ws = _workspace(x.device)
-        # algorithmic bytes: reduce reads dy, x (+ y for the mask); apply reads the same and writes dx (+ d residual)
-        ops = 2 * (2 + (y is not None)) + 1 + (dres_ptr is not None)
-        code = _timed("bn_bwd", N * H * W * C * 2 * ops, lambda: lib.moco_bn_bwd(
-            dy.data_ptr(), x.data_ptr(), y.data_ptr() if y is not None else None, N * H * W, C,
-            weight.data_ptr(), bias.data_ptr(), mean.data_ptr(), invstd.data_ptr(), int(ctx.relu),
-            int(ctx.has_res), dx.data_ptr(), dres_ptr, dgamma.data_ptr(), dbeta.data_ptr(),
-            ws.data_ptr(), ws.numel(), _lib.cur_stream()))
-        _lib.check(code, "moco_bn_bwd")
+            dres = dy                                             # without a ReLU the residual's gradient is dy itself
         return dx, dgamma, dbeta, dres, None, None, None, None, None, None, None
-
-
-def _layer(weight, bias, mean, invstd, stats=None, dgamma=None, dbeta=None):
-    """moco_bn_layer of one BatchNorm: stats = (running_mean, running_var, num_batches_tracked, momentum, eps)."""
-    ptr = lambda t: t.data_ptr() if t is not None else None
-    rm, rv, nbt, momentum, eps = stats if stats is not None else (None, None, None, 0.0, 0.0)
-    return _lib.BnLayer(ptr(weight), ptr(bias), ptr(rm), ptr(rv), ptr(nbt), float(momentum), float(eps), ptr(mean),
-                        ptr(invstd), ptr(dgamma), ptr(dbeta))
 
 
 class _BatchNormAddReluFn(torch.autograd.Function):
@@ -180,44 +229,12 @@ class _BatchNormAddReluFn(torch.autograd.Function):
         convolution (:func:`conv1x1_stats`), which also updated its running statistics; that statistics pass is
         skipped.  recompute: (a, w) with x = conv2d(a, w) of a 1x1 convolution (given required): y is computed from a
         by moco_conv1x1_bn_add_relu_fwd instead of reading x (:func:`conv1x1_bn_add_relu`)."""
-        lib = _lib.load()
         N, C, H, W = x.shape
-        M = N * H * W
         y = torch.empty_like(x)
-        mask = torch.empty((M, C // 8), dtype=torch.uint8, device=x.device) if want_mask else None
-        f32 = lambda: torch.empty(C, dtype=torch.float32, device=x.device)
-        mean, invstd = given if given is not None else (f32(), f32())
-        bn = _layer(weight, bias, mean, invstd, stats)
-        sc, sc_mean, sc_invstd = None, None, None
-        if sc_weight is not None:
-            sc_mean, sc_invstd = sc_given if sc_given is not None else (f32(), f32())
-            sc = _layer(sc_weight, sc_bias, sc_mean, sc_invstd, sc_stats)
-        ws = _workspace(x.device)
-        flags = (_lib.BN_STATS_GIVEN if given is not None else 0) | (_lib.BN_SC_STATS_GIVEN if sc_given is not None else 0)
-        # algorithmic bytes: statistics read x (+ the shortcut input) unless given; apply reads x and residual, writes
-        # y (+ mask bits)
-        passes = (given is None) + (sc is not None and sc_given is None)
-        nbytes = M * C * 2 * (3 + passes) + (M * C // 8 if want_mask else 0)
-        mask_ptr = mask.data_ptr() if mask is not None else None
-        if recompute is not None:
-            a, w = recompute
-            Cin = a.shape[1]
-            # algorithmic bytes: reads a, residual (+ the shortcut input for its statistics), writes y (+ mask bits)
-            nbytes = M * 2 * (Cin + C * (2 + passes)) + (M * C // 8 if want_mask else 0)
-            code = _timed("bn_fwd", nbytes, lambda: lib.moco_conv1x1_bn_add_relu_fwd(
-                a.data_ptr(), w.data_ptr(), residual.data_ptr(), y.data_ptr(), mask_ptr, M, Cin, C, bn, sc, flags,
-                ws.data_ptr(), ws.numel(), _lib.cur_stream()))
-            _lib.check(code, "moco_conv1x1_bn_add_relu_fwd")
-        elif flags:
-            code = _timed("bn_fwd", nbytes, lambda: lib.moco_bn_fwd_train_given(
-                x.data_ptr(), residual.data_ptr(), y.data_ptr(), mask_ptr, M, C, 1, bn, sc, flags, ws.data_ptr(),
-                ws.numel(), _lib.cur_stream()))
-            _lib.check(code, "moco_bn_fwd_train_given")
-        else:
-            code = _timed("bn_fwd", nbytes, lambda: lib.moco_bn_add_relu_fwd_train(
-                x.data_ptr(), residual.data_ptr(), y.data_ptr(), mask_ptr, M, C, bn, sc, ws.data_ptr(), ws.numel(),
-                _lib.cur_stream()))
-            _lib.check(code, "moco_bn_add_relu_fwd_train")
+        mask = torch.empty((N * H * W, C // 8), dtype=torch.uint8, device=x.device) if want_mask else None
+        sc = (sc_weight, sc_bias, sc_stats) if sc_weight is not None else None
+        mean, invstd, sc_mean, sc_invstd = _bn_fwd(x, residual, y, mask, True, (weight, bias, stats), sc, given,
+                                                   sc_given, recompute)
         ctx.save_for_backward(x, residual if sc is not None else None, mask, weight, mean, invstd, sc_weight, sc_mean,
                               sc_invstd)
         return y
@@ -227,51 +244,21 @@ class _BatchNormAddReluFn(torch.autograd.Function):
         x, residual, mask, weight, mean, invstd, sc_weight, sc_mean, sc_invstd = ctx.saved_tensors
         if mask is None:
             raise RuntimeError("moco_b200: BatchNormAct2d ran its forward without the ReLU mask (no input required grad)")
-        lib = _lib.load()
-        N, C, H, W = x.shape
-        M = N * H * W
         dy = _grad_rows(dy)
-        dx = torch.empty_like(x)
+        bn = (weight, None, mean, invstd)
         reduced, ctx.reduced = getattr(ctx, "reduced", None), None
         if reduced is not None and dy.data_ptr() == reduced[0].data_ptr():
             # the consumer's dgrad formed g = dy and the sums (_dgrad_bn_bwd); another consumer adding to the gradient
             # gives a different tensor, which takes the full backward below (g is already masked: mask(g + e) = g +
             # mask(e))
             g, dgamma, dbeta = reduced
-            bn = _layer(weight, None, mean, invstd, dgamma=dgamma, dbeta=dbeta)
-            # algorithmic bytes: reads g and x, writes dx
-            code = _timed("bn_bwd", M * C * 2 * 3, lambda: lib.moco_bn_bwd_apply_given(
-                g.data_ptr(), x.data_ptr(), None, M, C, bn, None, dx.data_ptr(), None, _lib.cur_stream()))
-            _lib.check(code, "moco_bn_bwd_apply_given")
+            dx = _bn_bwd(g, x, bn, False, sums=(dgamma, dbeta))[0]
             return (dx, g if ctx.needs_input_grad[1] else None, dgamma, dbeta, None, None, None, None, None, None, None,
                     None)
         dy2 = _take_handed(ctx)          # y's other consumer's gradient: summed inside both passes
-        f32 = lambda: torch.empty(C, dtype=torch.float32, device=x.device)
-        dgamma, dbeta = f32(), f32()
-        bn = _layer(weight, None, mean, invstd, dgamma=dgamma, dbeta=dbeta)
-        sc, sc_dgamma, sc_dbeta = None, None, None
-        if sc_weight is not None:
-            sc_dgamma, sc_dbeta = f32(), f32()
-            sc = _layer(sc_weight, None, sc_mean, sc_invstd, dgamma=sc_dgamma, dbeta=sc_dbeta)
-            dres = torch.empty_like(x)
-        else:
-            dres = torch.empty_like(x) if ctx.needs_input_grad[1] else None
-        ws = _workspace(x.device)
-        # algorithmic bytes: reduce reads dy (+ dy2), x, mask (+ shortcut input); apply reads the same and writes dx
-        # (+ d residual)
-        nbytes = (M * C * 2 * (5 + (dres is not None) + 2 * (sc is not None) + 2 * (dy2 is not None))
-                  + 2 * (M * C // 8))
-        ptr = lambda t: t.data_ptr() if t is not None else None
-        if dy2 is None:
-            code = _timed("bn_bwd", nbytes, lambda: lib.moco_bn_add_relu_bwd(
-                dy.data_ptr(), x.data_ptr(), ptr(residual), mask.data_ptr(), M, C, bn, sc, dx.data_ptr(), ptr(dres),
-                ws.data_ptr(), ws.numel(), _lib.cur_stream()))
-            _lib.check(code, "moco_bn_add_relu_bwd")
-        else:
-            code = _timed("bn_bwd", nbytes, lambda: lib.moco_bn_add_relu_bwd2(
-                dy.data_ptr(), dy2.data_ptr(), x.data_ptr(), ptr(residual), mask.data_ptr(), M, C, bn, sc,
-                dx.data_ptr(), ptr(dres), ws.data_ptr(), ws.numel(), _lib.cur_stream()))
-            _lib.check(code, "moco_bn_add_relu_bwd2")
+        sc = (sc_weight, sc_mean, sc_invstd, residual) if sc_weight is not None else None
+        dres = torch.empty_like(x) if sc is not None or ctx.needs_input_grad[1] else None
+        dx, dgamma, dbeta, sc_dgamma, sc_dbeta = _bn_bwd(dy, x, bn, True, mask=mask, dy2=dy2, sc=sc, dres=dres)
         return dx, dres, dgamma, dbeta, sc_dgamma, sc_dbeta, None, None, None, None, None, None
 
 
@@ -287,8 +274,7 @@ class _BatchNormReluMaxPoolFn(torch.autograd.Function):
         OH, OW = (H - 1) // 2 + 1, (W - 1) // 2 + 1
         y = torch.empty((N, C, OH, OW), dtype=x.dtype, device=x.device, memory_format=torch.channels_last)
         taps = torch.empty((N, OH, OW, C), dtype=torch.uint8, device=x.device)
-        mean = torch.empty(C, dtype=torch.float32, device=x.device)
-        invstd = torch.empty_like(mean)
+        mean, invstd = _f32(C, x.device), _f32(C, x.device)
         bn = _layer(weight, bias, mean, invstd, stats)
         ws = _workspace(x.device)
         # algorithmic bytes: statistics read x; the pool pass reads x, writes y and the tap bytes
@@ -315,16 +301,7 @@ class _BatchNormReluMaxPoolFn(torch.autograd.Function):
         else:
             _lib.check(lib.moco_maxpool3x3s2_bwd2(dy.data_ptr(), dy2.data_ptr(), taps.data_ptr(), g.data_ptr(), N, H, W,
                                                   C, _lib.cur_stream()), "moco_maxpool3x3s2_bwd2")
-        dx = torch.empty_like(x)
-        dgamma = torch.empty(C, dtype=torch.float32, device=x.device)
-        dbeta = torch.empty_like(dgamma)
-        ws = _workspace(x.device)
-        # algorithmic bytes: reduce reads g, x; apply reads g, x and writes dx
-        code = _timed("bn_bwd", N * H * W * C * 2 * 5, lambda: lib.moco_bn_bwd(
-            g.data_ptr(), x.data_ptr(), None, N * H * W, C, weight.data_ptr(), bias.data_ptr(), mean.data_ptr(),
-            invstd.data_ptr(), 1, 0, dx.data_ptr(), None, dgamma.data_ptr(), dbeta.data_ptr(), ws.data_ptr(),
-            ws.numel(), _lib.cur_stream()))
-        _lib.check(code, "moco_bn_bwd")
+        dx, dgamma, dbeta, _, _ = _bn_bwd(g, x, (weight, bias, mean, invstd), True)
         return dx, dgamma, dbeta, None
 
 
@@ -373,8 +350,7 @@ class _Conv1x1StatsFn(torch.autograd.Function):
         N, Cin, H, W = x.shape
         Cout = w.shape[0]
         y = torch.empty((N, Cout, H, W), dtype=torch.bfloat16, device=x.device, memory_format=torch.channels_last)
-        mean = torch.empty(Cout, dtype=torch.float32, device=x.device)
-        invstd = torch.empty_like(mean)
+        mean, invstd = _f32(Cout, x.device), _f32(Cout, x.device)
         ws = _workspace(x.device, conv=True)
         _lib.check(lib.moco_conv1x1_bn_stats(x.data_ptr(), w.data_ptr(), y.data_ptr(), N * H * W, Cin, Cout,
                                              _layer(None, None, mean, invstd, stats), ws.data_ptr(), ws.numel(),
@@ -400,11 +376,13 @@ class _Conv1x1StatsFn(torch.autograd.Function):
 # SXM at a 700 W power limit (tools/conv1x1_dgrad_times.py, results/conv1x1_dgrad_times_h100.json).  These are all
 # such shapes that also run their forward on moco_conv1x1_bn_stats (_CONV1X1_WINS).
 _DGRAD_WINS = frozenset({(256, 64), (256, 128), (512, 128), (512, 256)})
+# the fewest rows N * H * W of a shape in the _*_WINS tables at the batch they were measured at: 256 x 14 x 14
+_BATCH256_ROWS = 50176
 
 
 def _dgrad_wins(M, Cin, Cout):
     """The shapes moco_conv1x1_dgrad_bn_bwd was measured to win on (_DGRAD_WINS) at batch 256's row counts."""
-    return M >= 50176 and (Cin, Cout) in _DGRAD_WINS
+    return M >= _BATCH256_ROWS and (Cin, Cout) in _DGRAD_WINS
 
 
 def _dgrad_bn_bwd(node, dh, w):
@@ -424,8 +402,7 @@ def _dgrad_bn_bwd(node, dh, w):
     dy2 = _take_handed(node)
     dh = _grad_rows(dh)
     g = torch.empty_like(x)
-    dgamma = torch.empty(C, dtype=torch.float32, device=x.device)
-    dbeta = torch.empty_like(dgamma)
+    dgamma, dbeta = _f32(C, x.device), _f32(C, x.device)
     ws = _workspace(x.device, conv=True)
     _lib.check(lib.moco_conv1x1_dgrad_bn_bwd(
         dh.data_ptr(), w.data_ptr(), g.data_ptr(), M, C, Cout, x.data_ptr(), mask.data_ptr(), dy2.data_ptr(), None,
@@ -447,7 +424,7 @@ _CONV1X1_WINS = frozenset({(64, 64), (256, 64), (64, 256), (256, 128), (512, 128
 def _conv1x1_wins(M, Cin, Cout):
     """The shapes moco_conv1x1_bn_stats was measured to win on (_CONV1X1_WINS) at batch 256's row counts; smaller
     batches were not measured and keep cuDNN."""
-    return M >= 50176 and (Cin, Cout) in _CONV1X1_WINS
+    return M >= _BATCH256_ROWS and (Cin, Cout) in _CONV1X1_WINS
 
 
 def _conv1x1_ok(conv, bn, x, residual=None, shortcut_bn=None):
@@ -503,7 +480,7 @@ _APPLY_WINS = frozenset({(64, 256, False, False), (128, 512, False, False), (256
 
 
 def _apply_wins(M, Cin, Cout, key, shortcut):
-    return M >= 50176 and (Cin, Cout, key, shortcut) in _APPLY_WINS
+    return M >= _BATCH256_ROWS and (Cin, Cout, key, shortcut) in _APPLY_WINS
 
 
 def conv1x1_bn_add_relu(conv, bn, x, residual, shortcut_bn=None, sc_stats=None, avgpool=False):
@@ -532,26 +509,10 @@ def conv1x1_bn_add_relu(conv, bn, x, residual, shortcut_bn=None, sc_stats=None, 
 def _conv_bn_add_relu_nograd(x, w, bn, residual, shortcut_bn, sc_stats):
     """relu(bn(conv2d(x, w)) + r) for a forward without a backward: one moco_conv1x1_bn_add_relu_fwd call runs the
     statistics pass (no store) and the recomputing apply pass, plus the shortcut BN's statistics unless given."""
-    lib = _lib.load()
     N, Cin, H, W = x.shape
-    C, M = w.shape[0], N * H * W
-    y = torch.empty((N, C, H, W), dtype=torch.bfloat16, device=x.device, memory_format=torch.channels_last)
-    f32 = lambda: torch.empty(C, dtype=torch.float32, device=x.device)
-    mean, invstd = f32(), f32()                     # kept alive until the call: the layer holds raw pointers
-    layer = _layer(bn.weight, bn.bias, mean, invstd, bn._stats())
-    sc, flags = None, 0
-    if shortcut_bn is not None:
-        sc_mean, sc_invstd = sc_stats if sc_stats is not None else (f32(), f32())
-        sc = _layer(shortcut_bn.weight, shortcut_bn.bias, sc_mean, sc_invstd, shortcut_bn._stats())
-        flags = _lib.BN_SC_STATS_GIVEN if sc_stats is not None else 0
-    ws = _workspace(x.device)
-    # algorithmic bytes: both passes read x; the apply reads the residual (+ the shortcut input for its statistics)
-    # and writes y
-    nbytes = M * 2 * (2 * Cin + C * (2 + (sc is not None and sc_stats is None)))
-    code = _timed("bn_fwd", nbytes, lambda: lib.moco_conv1x1_bn_add_relu_fwd(
-        x.data_ptr(), w.data_ptr(), residual.data_ptr(), y.data_ptr(), None, M, Cin, C, layer, sc, flags,
-        ws.data_ptr(), ws.numel(), _lib.cur_stream()))
-    _lib.check(code, "moco_conv1x1_bn_add_relu_fwd")
+    y = torch.empty((N, w.shape[0], H, W), dtype=torch.bfloat16, device=x.device, memory_format=torch.channels_last)
+    sc = (shortcut_bn.weight, shortcut_bn.bias, shortcut_bn._stats()) if shortcut_bn is not None else None
+    _bn_fwd(None, residual, y, None, True, (bn.weight, bn.bias, bn._stats()), sc, None, sc_stats, recompute=(x, w))
     return y
 
 
@@ -568,24 +529,24 @@ class BatchNormAct2d(nn.BatchNorm2d):
     def _fusable(self, x, residual):
         return _rows_ok(x) and self._fusable_shape(x.shape, residual)
 
+    def _envelope_ok(self, shape):
+        """What the training and the frozen kernels both need of the module and of the input's channels."""
+        C = self.num_features
+        return (_enabled and self.affine and 64 <= C <= 2048 and (C & (C - 1)) == 0 and shape[1] == C
+                and self.weight.dtype == torch.float32 and self.weight.is_cuda)
+
     def _fusable_shape(self, shape, residual):
         """The training kernels take a bf16 channels_last input of this shape (and this residual)."""
-        C = self.num_features
-        return (_enabled and self.training and self.affine and self.momentum is not None
+        return (self._envelope_ok(shape) and self.training and self.momentum is not None
                 and (residual is None or (_rows_ok(residual) and residual.shape == shape))
-                and 64 <= C <= 2048 and (C & (C - 1)) == 0 and shape[1] == C
-                and shape.numel() // C > 1             # a single value per channel: nn.BatchNorm2d's own error
-                and self.weight.dtype == torch.float32 and self.weight.is_cuda
+                and shape.numel() // self.num_features > 1    # a single value per channel: nn.BatchNorm2d's own error
                 and (self.running_mean is None or self.running_mean.dtype == torch.float32))
 
     def _eval_ok(self, x, residual):
         """The frozen path: eval mode, grad mode off, running statistics, and activations the kernels take."""
-        C = self.num_features
-        return (_enabled and self.frozen and not self.training and not torch.is_grad_enabled() and self.affine
+        return (self.frozen and not self.training and not torch.is_grad_enabled()
                 and self.track_running_stats and self.running_mean is not None
-                and _rows_ok(x) and (residual is None or _rows_ok(residual, x))
-                and 64 <= C <= 2048 and (C & (C - 1)) == 0 and x.shape[1] == C
-                and self.weight.dtype == torch.float32 and self.weight.is_cuda
+                and _rows_ok(x) and (residual is None or _rows_ok(residual, x)) and self._envelope_ok(x.shape)
                 and self.running_var.dtype == torch.float32)
 
     def folded(self):
@@ -608,20 +569,19 @@ class BatchNormAct2d(nn.BatchNorm2d):
         N, C, H, W = x.shape
         scale, shift = self.folded()
         sc_scale, sc_shift = sc.folded() if sc is not None else (None, None)
-        ptr = lambda t: t.data_ptr() if t is not None else None
         # algorithmic bytes: reads x (+ residual), writes y (or the pooled fp32 features)
         reads = N * H * W * C * 2 * (1 + (residual is not None))
         if avgpool:
             y = torch.empty((N, C), dtype=torch.float32, device=x.device)
             code = _timed("bn_eval", reads + N * C * 4, lambda: lib.moco_bn_eval_act_avgpool(
-                x.data_ptr(), ptr(residual), y.data_ptr(), N, H * W, C, scale.data_ptr(), shift.data_ptr(),
-                int(self.relu), ptr(sc_scale), ptr(sc_shift), _lib.cur_stream()))
+                x.data_ptr(), _ptr(residual), y.data_ptr(), N, H * W, C, scale.data_ptr(), shift.data_ptr(),
+                int(self.relu), _ptr(sc_scale), _ptr(sc_shift), _lib.cur_stream()))
             _lib.check(code, "moco_bn_eval_act_avgpool")
             return y
         y = torch.empty_like(x)
         code = _timed("bn_eval", reads + N * H * W * C * 2, lambda: lib.moco_bn_eval_act(
-            x.data_ptr(), ptr(residual), y.data_ptr(), N * H * W, C, scale.data_ptr(), shift.data_ptr(),
-            int(self.relu), ptr(sc_scale), ptr(sc_shift), _lib.cur_stream()))
+            x.data_ptr(), _ptr(residual), y.data_ptr(), N * H * W, C, scale.data_ptr(), shift.data_ptr(),
+            int(self.relu), _ptr(sc_scale), _ptr(sc_shift), _lib.cur_stream()))
         _lib.check(code, "moco_bn_eval_act")
         return y
 
@@ -712,9 +672,7 @@ class _MaxPool3x3s2Fn(torch.autograd.Function):
     def backward(ctx, dy):
         (taps,) = ctx.saved_tensors
         N, C, H, W = ctx.shape
-        if dy.dtype != torch.bfloat16:
-            dy = dy.to(torch.bfloat16)
-        dy = dy.contiguous(memory_format=torch.channels_last)
+        dy = _grad_rows(dy)
         dx = torch.empty((N, C, H, W), dtype=torch.bfloat16, device=dy.device, memory_format=torch.channels_last)
         _lib.check(_lib.load().moco_maxpool3x3s2_bwd(dy.data_ptr(), taps.data_ptr(), dx.data_ptr(), N, H, W, C,
                                                      _lib.cur_stream()), "moco_maxpool3x3s2_bwd")

@@ -609,150 +609,87 @@ static cudaError_t run_bwd_apply(BnBwdApplyArgs& p, cudaStream_t stream) {
     return cudaGetLastError();
 }
 
-static cudaError_t stats_pass(const void* x, long long M, int C, float* running_mean, float* running_var, long long* nbt,
-                              float momentum, float eps, float* save_mean, float* save_invstd, void* ws,
-                              cudaStream_t stream) {
+cudaError_t launch_bn_stats(const void* x, long long M, int C, const BnLayer& bn, void* ws, cudaStream_t stream) {
+    if (!bn_shape_ok(M, C)) return cudaErrorNotSupported;
     BnStatsArgs s{};
     s.x = static_cast<const uint4*>(x);
     s.M = M; s.C = C;
-    s.eps = eps; s.momentum = momentum;
-    s.counters = static_cast<unsigned int*>(ws);
-    s.partial = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 256);
-    s.mean = save_mean; s.invstd = save_invstd;
-    s.running_mean = running_mean; s.running_var = running_var; s.num_batches_tracked = nbt;
+    s.eps = bn.eps; s.momentum = bn.momentum;
+    s.counters = static_cast<unsigned int*>(ws); s.partial = bn_ws_partials(ws);
+    s.mean = bn.save_mean; s.invstd = bn.save_invstd;
+    s.running_mean = bn.running_mean; s.running_var = bn.running_var; s.num_batches_tracked = bn.num_batches_tracked;
     return run_stats<kBnStatsUnroll, kBnStatsCtas>(s, stream);
 }
 
-cudaError_t launch_bn_stats(const void* x, long long M, int C, const BnLayer& bn, void* ws, cudaStream_t stream) {
-    if (!bn_shape_ok(M, C)) return cudaErrorNotSupported;
-    return stats_pass(x, M, C, bn.running_mean, bn.running_var, bn.num_batches_tracked, bn.momentum, bn.eps,
-                      bn.save_mean, bn.save_invstd, ws, stream);
-}
-
-cudaError_t launch_bn_fwd_train(const void* x, const void* res, void* y, long long M, int C, const float* gamma,
-                                const float* beta, float* running_mean, float* running_var, long long* nbt, float momentum,
-                                float eps, int relu, float* save_mean, float* save_invstd, void* ws, cudaStream_t stream) {
-    if (!bn_shape_ok(M, C)) return cudaErrorNotSupported;
-    cudaError_t e = stats_pass(x, M, C, running_mean, running_var, nbt, momentum, eps, save_mean, save_invstd, ws, stream);
-    if (e != cudaSuccess) return e;
-    BnApplyArgs p{};
-    p.x = static_cast<const uint4*>(x); p.res = static_cast<const uint4*>(res); p.y = static_cast<uint4*>(y);
-    p.V = M * (C >> 3); p.C = C; p.relu = relu;
-    p.mean = save_mean; p.invstd = save_invstd; p.gamma = gamma; p.beta = beta;
-    return run_apply<kBnApplyUnroll, kBnApplyCtas, false>(p, stream);
-}
-
-cudaError_t launch_bn_bwd(const void* dy, const void* x, const void* y, long long M, int C, const float* gamma,
-                          const float* beta, const float* save_mean, const float* save_invstd, int relu, int has_residual,
-                          void* dx, void* dres, float* dgamma, float* dbeta, void* ws, cudaStream_t stream) {
-    if (!bn_shape_ok(M, C)) return cudaErrorNotSupported;
-    const int mask = !relu ? kMaskNone : (has_residual ? kMaskFromY : kMaskFromX);
-    if (mask == kMaskFromY && y == nullptr) return cudaErrorInvalidValue;
-    BnBwdReduceArgs s{};
-    s.dy = static_cast<const uint4*>(dy); s.x = static_cast<const uint4*>(x); s.y = static_cast<const uint4*>(y);
-    s.M = M; s.C = C; s.mask = mask;
-    s.counters = static_cast<unsigned int*>(ws);
-    s.partial = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 256);
-    s.mean = save_mean; s.invstd = save_invstd; s.gamma = gamma; s.beta = beta;
-    s.sum_dy = dbeta; s.sum_dy_xhat = dgamma;
-    cudaError_t e = run_bwd_reduce<kBnBwdReduceUnroll, kBnBwdReduceCtas, false>(s, stream);
-    if (e != cudaSuccess) return e;
-    BnBwdApplyArgs p{};
-    p.dy = s.dy; p.x = s.x; p.y = s.y; p.dx = static_cast<uint4*>(dx); p.dres = static_cast<uint4*>(dres);
-    p.V = M * (C >> 3); p.C = C; p.mask = mask; p.inv_m = (float)(1.0 / (double)M);
-    p.mean = save_mean; p.invstd = save_invstd; p.gamma = gamma; p.beta = beta;
-    p.sum_dy = dbeta; p.sum_dy_xhat = dgamma;
-    return run_bwd_apply<kBnBwdApplyUnroll, kBnBwdApplyCtas, false>(p, stream);
-}
-
-cudaError_t launch_bn_fwd_given(const void* x, const void* res, void* y, void* mask, long long M, int C, int relu,
-                                const BnLayer& bn, const BnLayer* sc, int given, void* ws, cudaStream_t stream) {
-    if (!bn_shape_ok(M, C)) return cudaErrorNotSupported;
+cudaError_t launch_bn_fwd(const BnFwdPlan& f, cudaStream_t stream) {
+    if (!bn_shape_ok(f.M, f.C)) return cudaErrorNotSupported;
+    const BnLayer& bn = *f.bn;
+    const BnLayer* sc = f.sc;
     cudaError_t e = cudaSuccess;
-    if (!(given & MOCO_BN_STATS_GIVEN))
-        e = stats_pass(x, M, C, bn.running_mean, bn.running_var, bn.num_batches_tracked, bn.momentum, bn.eps,
-                       bn.save_mean, bn.save_invstd, ws, stream);
-    if (e == cudaSuccess && sc != nullptr && !(given & MOCO_BN_SC_STATS_GIVEN))
-        e = stats_pass(res, M, C, sc->running_mean, sc->running_var, sc->num_batches_tracked, sc->momentum, sc->eps,
-                       sc->save_mean, sc->save_invstd, ws, stream);
+    if (!(f.given & MOCO_BN_STATS_GIVEN)) e = launch_bn_stats(f.x, f.M, f.C, bn, f.ws, stream);
+    if (e == cudaSuccess && sc != nullptr && !(f.given & MOCO_BN_SC_STATS_GIVEN))
+        e = launch_bn_stats(f.res, f.M, f.C, *sc, f.ws, stream);
     if (e != cudaSuccess) return e;
     BnApplyArgs p{};
-    p.x = static_cast<const uint4*>(x); p.res = static_cast<const uint4*>(res); p.y = static_cast<uint4*>(y);
-    p.mask = static_cast<uint8_t*>(mask);
-    p.V = M * (C >> 3); p.C = C; p.relu = relu;
+    p.x = static_cast<const uint4*>(f.x); p.res = static_cast<const uint4*>(f.res); p.y = static_cast<uint4*>(f.y);
+    p.mask = static_cast<uint8_t*>(f.mask);
+    p.V = f.M * (f.C >> 3); p.C = f.C; p.relu = f.relu;
     p.mean = bn.save_mean; p.invstd = bn.save_invstd; p.gamma = bn.gamma; p.beta = bn.beta;
     if (sc == nullptr) return run_apply<kBnApplyUnroll, kBnApplyCtas, false>(p, stream);
     p.mean2 = sc->save_mean; p.invstd2 = sc->save_invstd; p.gamma2 = sc->gamma; p.beta2 = sc->beta;
     return run_apply<kBnApplyUnroll, kBnApplyCtas, true>(p, stream);
 }
 
-cudaError_t launch_bn_add_relu_fwd(const void* x, const void* res, void* y, void* mask, long long M, int C,
-                                   const BnLayer& bn, const BnLayer* sc, void* ws, cudaStream_t stream) {
-    return launch_bn_fwd_given(x, res, y, mask, M, C, 1, bn, sc, 0, ws, stream);
-}
-
 template <bool SUM>
-static cudaError_t add_relu_bwd(BnBwdReduceArgs& s, BnBwdApplyArgs& p, const BnLayer* sc, void* dres,
-                                cudaStream_t stream) {
-    cudaError_t e;
-    if (sc == nullptr) {
-        p.dres = static_cast<uint4*>(dres);
-        e = run_bwd_reduce<kBnBwdReduceUnroll, kBnBwdReduceCtas, false, SUM>(s, stream);
-        if (e != cudaSuccess) return e;
-        if constexpr (SUM) return run_bwd_apply<kBnBwdApplySumUnroll, kBnBwdApplySumCtas, false, true>(p, stream);
-        return run_bwd_apply<kBnBwdApplyUnroll, kBnBwdApplyCtas, false, false>(p, stream);
-    }
-    s.x2 = p.x2;
-    s.mean2 = sc->save_mean; s.invstd2 = sc->save_invstd;
-    s.sum_dy2 = sc->dbeta; s.sum_dy_xhat2 = sc->dgamma;
-    e = run_bwd_reduce<kBnBwdReduceUnroll, kBnBwdReduceCtas, true, SUM>(s, stream);
+static cudaError_t bwd_passes(BnBwdReduceArgs& s, BnBwdApplyArgs& p, bool shortcut, bool reduce, cudaStream_t stream) {
+    cudaError_t e = cudaSuccess;
+    if (reduce)
+        e = shortcut ? run_bwd_reduce<kBnBwdReduceUnroll, kBnBwdReduceCtas, true, SUM>(s, stream)
+                     : run_bwd_reduce<kBnBwdReduceUnroll, kBnBwdReduceCtas, false, SUM>(s, stream);
     if (e != cudaSuccess) return e;
-    p.dx2 = static_cast<uint4*>(dres);
-    p.mean2 = sc->save_mean; p.invstd2 = sc->save_invstd; p.gamma2 = sc->gamma; p.sum_dy_xhat2 = sc->dgamma;
-    return run_bwd_apply<kBnBwdApplyScUnroll, kBnBwdApplyScCtas, true, SUM>(p, stream);
+    if (shortcut) return run_bwd_apply<kBnBwdApplyScUnroll, kBnBwdApplyScCtas, true, SUM>(p, stream);
+    if constexpr (SUM) return run_bwd_apply<kBnBwdApplySumUnroll, kBnBwdApplySumCtas, false, true>(p, stream);
+    return run_bwd_apply<kBnBwdApplyUnroll, kBnBwdApplyCtas, false, false>(p, stream);
 }
 
-cudaError_t launch_bn_add_relu_bwd(const void* dy, const void* dy2, const void* x, const void* res, const void* mask,
-                                   long long M, int C, const BnLayer& bn, const BnLayer* sc, void* dx, void* dres,
-                                   void* ws, cudaStream_t stream) {
-    if (!bn_shape_ok(M, C)) return cudaErrorNotSupported;
+cudaError_t launch_bn_bwd(const BnBwdPlan& b, cudaStream_t stream) {
+    // apply only with a shortcut BN is not taken: its apply kernel reads the mask bits (kShortcut), and
+    // moco_conv1x1_dgrad_bn_bwd does not produce a downsample block's g
+    if (!bn_shape_ok(b.M, b.C) || (b.reduced && b.sc != nullptr)) return cudaErrorNotSupported;
+    const int mask = b.mbits != nullptr ? kMaskFromBits
+                                        : (!b.relu ? kMaskNone : (b.has_residual ? kMaskFromY : kMaskFromX));
+    if (mask == kMaskFromY && b.y == nullptr) return cudaErrorInvalidValue;
+    const BnLayer& bn = *b.bn;
+    const BnLayer* sc = b.sc;
     BnBwdReduceArgs s{};
-    s.dy = static_cast<const uint4*>(dy); s.dy2 = static_cast<const uint4*>(dy2); s.x = static_cast<const uint4*>(x);
-    s.mbits = static_cast<const uint8_t*>(mask);
-    s.M = M; s.C = C; s.mask = kMaskFromBits;
-    s.counters = static_cast<unsigned int*>(ws);
-    s.partial = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 256);
-    s.mean = bn.save_mean; s.invstd = bn.save_invstd; s.gamma = bn.gamma;
+    s.dy = static_cast<const uint4*>(b.dy); s.dy2 = static_cast<const uint4*>(b.dy2); s.x = static_cast<const uint4*>(b.x);
+    s.y = static_cast<const uint4*>(b.y); s.mbits = static_cast<const uint8_t*>(b.mbits);
+    s.M = b.M; s.C = b.C; s.mask = mask;
+    s.counters = static_cast<unsigned int*>(b.ws); s.partial = bn_ws_partials(b.ws);
+    s.mean = bn.save_mean; s.invstd = bn.save_invstd; s.gamma = bn.gamma; s.beta = bn.beta;
     s.sum_dy = bn.dbeta; s.sum_dy_xhat = bn.dgamma;
     BnBwdApplyArgs p{};
-    p.dy = s.dy; p.dy2 = s.dy2; p.x = s.x; p.mbits = s.mbits; p.dx = static_cast<uint4*>(dx);
-    p.x2 = static_cast<const uint4*>(res);
-    p.V = M * (C >> 3); p.C = C; p.mask = kMaskFromBits; p.inv_m = (float)(1.0 / (double)M);
-    p.mean = bn.save_mean; p.invstd = bn.save_invstd; p.gamma = bn.gamma;
+    p.dy = s.dy; p.dy2 = s.dy2; p.x = s.x; p.y = s.y; p.mbits = s.mbits; p.dx = static_cast<uint4*>(b.dx);
+    p.V = b.M * (b.C >> 3); p.C = b.C; p.mask = mask; p.inv_m = (float)(1.0 / (double)b.M);
+    p.mean = bn.save_mean; p.invstd = bn.save_invstd; p.gamma = bn.gamma; p.beta = bn.beta;
     p.sum_dy = bn.dbeta; p.sum_dy_xhat = bn.dgamma;
-    return dy2 != nullptr ? add_relu_bwd<true>(s, p, sc, dres, stream) : add_relu_bwd<false>(s, p, sc, dres, stream);
-}
-
-cudaError_t launch_bn_bwd_apply_given(const void* g, const void* x, const void* x2, long long M, int C, const BnLayer& bn,
-                                      const BnLayer* sc, void* dx, void* dx2, cudaStream_t stream) {
-    // a shortcut BN (x2, dx2) is not taken: its apply kernel reads the mask bits (kShortcut), and
-    // moco_conv1x1_dgrad_bn_bwd does not produce a downsample block's g
-    (void)x2; (void)dx2;
-    if (!bn_shape_ok(M, C) || sc != nullptr) return cudaErrorNotSupported;
-    BnBwdApplyArgs p{};
-    p.dy = static_cast<const uint4*>(g); p.x = static_cast<const uint4*>(x); p.dx = static_cast<uint4*>(dx);
-    p.V = M * (C >> 3); p.C = C; p.mask = kMaskNone; p.inv_m = (float)(1.0 / (double)M);
-    p.mean = bn.save_mean; p.invstd = bn.save_invstd; p.gamma = bn.gamma;
-    p.sum_dy = bn.dbeta; p.sum_dy_xhat = bn.dgamma;
-    return run_bwd_apply<kBnBwdApplyUnroll, kBnBwdApplyCtas, false>(p, stream);
+    if (sc == nullptr) {
+        p.dres = static_cast<uint4*>(b.dres);
+    } else {
+        s.x2 = p.x2 = static_cast<const uint4*>(b.x2);
+        p.dx2 = static_cast<uint4*>(b.dres);
+        s.mean2 = p.mean2 = sc->save_mean; s.invstd2 = p.invstd2 = sc->save_invstd;
+        s.sum_dy2 = sc->dbeta; s.sum_dy_xhat2 = sc->dgamma;
+        p.gamma2 = sc->gamma; p.sum_dy_xhat2 = sc->dgamma;
+    }
+    return b.dy2 != nullptr ? bwd_passes<true>(s, p, sc != nullptr, !b.reduced, stream)
+                            : bwd_passes<false>(s, p, sc != nullptr, !b.reduced, stream);
 }
 
 cudaError_t launch_bn_relu_maxpool_fwd(const void* x, void* y, void* taps, int N, int H, int W, int C, const BnLayer& bn,
                                        void* ws, cudaStream_t stream) {
-    const long long M = (long long)N * H * W;
-    if (N < 1 || H < 1 || W < 1 || !bn_shape_ok(M, C)) return cudaErrorNotSupported;
-    cudaError_t e = stats_pass(x, M, C, bn.running_mean, bn.running_var, bn.num_batches_tracked, bn.momentum, bn.eps,
-                               bn.save_mean, bn.save_invstd, ws, stream);
+    if (N < 1 || H < 1 || W < 1) return cudaErrorNotSupported;
+    cudaError_t e = launch_bn_stats(x, (long long)N * H * W, C, bn, ws, stream);
     if (e != cudaSuccess) return e;
     return launch_maxpool_fwd(x, y, taps, N, H, W, C, stream, bn.save_mean, bn.save_invstd, bn.gamma, bn.beta);
 }

@@ -51,6 +51,32 @@ static inline void prof_mark(int kernel, int which, cudaStream_t s) {
 
 // the kernels' 16-byte vector loads and stores need it; NULL counts as aligned (the caller checks for NULL)
 static bool misaligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
+// a required activation / workspace pointer: not NULL, and aligned for the kernels' 16-byte vectors
+static bool ptr16(const void* p) { return p && !misaligned16(p); }
+
+static int bn_bad_argument(const char* fn, const char* what) {
+    set_error("%s: bad argument (%s)", fn, what);
+    return MOCO_ERR_INVALID;
+}
+
+// What every training BatchNorm entry point does once its arguments are checked: the workspace check (reduces: a
+// statistics / reduction pass runs), the launch of its plan, and the mapping of the launcher's refusals.
+template <typename Plan>
+static int bn_launch(const char* fn, cudaError_t (*launch)(const Plan&, cudaStream_t), const Plan& plan, bool reduces,
+                     size_t workspace_bytes, void* stream_) {
+    if (reduces && workspace_bytes < bn_workspace_bytes()) {
+        set_error("%s: workspace too small", fn);
+        return MOCO_ERR_WORKSPACE;
+    }
+    const cudaError_t e = launch(plan, static_cast<cudaStream_t>(stream_));
+    if (e == cudaErrorNotSupported) {
+        set_error("%s: needs M >= 1 and C a power of two in [64, 2048]; moco_bn_bwd_apply_given takes no shortcut BN "
+                  "(M=%lld C=%d)", fn, plan.M, plan.C);
+        return MOCO_ERR_UNSUPPORTED;
+    }
+    if (e != cudaSuccess) return cuda_fail(fn, e);
+    return MOCO_OK;
+}
 
 }  // namespace moco
 
@@ -540,48 +566,6 @@ int moco_maxpool3x3s2_bwd2(const void* dy, const void* dy2, const void* taps, vo
 
 size_t moco_bn_workspace_bytes(void) { return bn_workspace_bytes(); }
 
-int moco_bn_fwd_train(const void* x, const void* residual, void* y, long long M, int C, const float* gamma,
-                      const float* beta, float* running_mean, float* running_var, long long* num_batches_tracked,
-                      float momentum, float eps, int relu, float* save_mean, float* save_invstd, void* workspace,
-                      size_t workspace_bytes, void* stream_) {
-    g_err[0] = 0;
-    if (!x || !y || !gamma || !beta || !save_mean || !save_invstd || !workspace || (running_mean == nullptr) != (running_var == nullptr) ||
-        misaligned16(x) || misaligned16(y) || misaligned16(residual) || misaligned16(workspace) || x == y || !(eps > 0.f)) {
-        set_error("moco_bn_fwd_train: bad argument (null / misaligned pointer, in-place, eps <= 0)");
-        return MOCO_ERR_INVALID;
-    }
-    if (workspace_bytes < bn_workspace_bytes()) { set_error("moco_bn_fwd_train: workspace too small"); return MOCO_ERR_WORKSPACE; }
-    cudaError_t e = launch_bn_fwd_train(x, residual, y, M, C, gamma, beta, running_mean, running_var, num_batches_tracked,
-                                        momentum, eps, relu, save_mean, save_invstd, workspace, static_cast<cudaStream_t>(stream_));
-    if (e == cudaErrorNotSupported) {
-        set_error("moco_bn_fwd_train: needs M >= 1 and C a power of two in [64, 2048] (M=%lld C=%d)", M, C);
-        return MOCO_ERR_UNSUPPORTED;
-    }
-    if (e != cudaSuccess) return cuda_fail("batch-norm forward kernels", e);
-    return MOCO_OK;
-}
-
-int moco_bn_bwd(const void* dy, const void* x, const void* y, long long M, int C, const float* gamma, const float* beta,
-                const float* save_mean, const float* save_invstd, int relu, int has_residual, void* dx, void* dresidual,
-                float* dgamma, float* dbeta, void* workspace, size_t workspace_bytes, void* stream_) {
-    g_err[0] = 0;
-    if (!dy || !x || !dx || !gamma || !beta || !save_mean || !save_invstd || !dgamma || !dbeta || !workspace ||
-        (relu && has_residual && !y) || misaligned16(dy) || misaligned16(x) || misaligned16(y) || misaligned16(dx) ||
-        misaligned16(dresidual) || misaligned16(workspace)) {
-        set_error("moco_bn_bwd: bad argument (null / misaligned pointer; y is required with relu + residual)");
-        return MOCO_ERR_INVALID;
-    }
-    if (workspace_bytes < bn_workspace_bytes()) { set_error("moco_bn_bwd: workspace too small"); return MOCO_ERR_WORKSPACE; }
-    cudaError_t e = launch_bn_bwd(dy, x, y, M, C, gamma, beta, save_mean, save_invstd, relu, has_residual, dx, dresidual,
-                                  dgamma, dbeta, workspace, static_cast<cudaStream_t>(stream_));
-    if (e == cudaErrorNotSupported) {
-        set_error("moco_bn_bwd: needs M >= 1 and C a power of two in [64, 2048] (M=%lld C=%d)", M, C);
-        return MOCO_ERR_UNSUPPORTED;
-    }
-    if (e != cudaSuccess) return cuda_fail("batch-norm backward kernels", e);
-    return MOCO_OK;
-}
-
 static bool bn_layer_fwd_ok(const moco_bn_layer* b) {
     return b && b->gamma && b->beta && b->save_mean && b->save_invstd &&
            (b->running_mean == nullptr) == (b->running_var == nullptr) && b->eps > 0.f;
@@ -591,25 +575,48 @@ static bool bn_layer_bwd_ok(const moco_bn_layer* b) {
     return b && b->gamma && b->save_mean && b->save_invstd && b->dgamma && b->dbeta;
 }
 
+int moco_bn_fwd_train(const void* x, const void* residual, void* y, long long M, int C, const float* gamma,
+                      const float* beta, float* running_mean, float* running_var, long long* num_batches_tracked,
+                      float momentum, float eps, int relu, float* save_mean, float* save_invstd, void* workspace,
+                      size_t workspace_bytes, void* stream_) {
+    g_err[0] = 0;
+    const moco_bn_layer bn = {gamma, beta, running_mean, running_var, num_batches_tracked, momentum, eps, save_mean,
+                              save_invstd, nullptr, nullptr};
+    if (!ptr16(x) || !ptr16(y) || !ptr16(workspace) || !bn_layer_fwd_ok(&bn) || misaligned16(residual) || x == y)
+        return bn_bad_argument("moco_bn_fwd_train", "null / misaligned pointer, in-place, eps <= 0");
+    BnFwdPlan f{};
+    f.x = x; f.res = residual; f.y = y; f.ws = workspace; f.bn = &bn; f.M = M; f.C = C; f.relu = relu;
+    return bn_launch("moco_bn_fwd_train", launch_bn_fwd, f, true, workspace_bytes, stream_);
+}
+
+int moco_bn_bwd(const void* dy, const void* x, const void* y, long long M, int C, const float* gamma, const float* beta,
+                const float* save_mean, const float* save_invstd, int relu, int has_residual, void* dx, void* dresidual,
+                float* dgamma, float* dbeta, void* workspace, size_t workspace_bytes, void* stream_) {
+    g_err[0] = 0;
+    // the backward only reads the saved statistics
+    const moco_bn_layer bn = {gamma, beta, nullptr, nullptr, nullptr, 0.f, 0.f, const_cast<float*>(save_mean),
+                              const_cast<float*>(save_invstd), dgamma, dbeta};
+    if (!ptr16(dy) || !ptr16(x) || !ptr16(dx) || !ptr16(workspace) || !bn_layer_bwd_ok(&bn) || !beta ||
+        (relu && has_residual && !y) || misaligned16(y) || misaligned16(dresidual))
+        return bn_bad_argument("moco_bn_bwd", "null / misaligned pointer; y is required with relu + residual");
+    BnBwdPlan b{};
+    b.dy = dy; b.x = x; b.y = y; b.dx = dx; b.dres = dresidual; b.ws = workspace; b.bn = &bn;
+    b.M = M; b.C = C; b.relu = relu; b.has_residual = has_residual;
+    return bn_launch("moco_bn_bwd", launch_bn_bwd, b, true, workspace_bytes, stream_);
+}
+
 int moco_bn_add_relu_fwd_train(const void* x, const void* residual, void* y, void* mask, long long M, int C,
                                const moco_bn_layer* bn, const moco_bn_layer* shortcut, void* workspace,
                                size_t workspace_bytes, void* stream_) {
     g_err[0] = 0;
-    if (!x || !residual || !y || !workspace || !bn_layer_fwd_ok(bn) || (shortcut && !bn_layer_fwd_ok(shortcut)) ||
-        misaligned16(x) || misaligned16(residual) || misaligned16(y) || misaligned16(workspace) || x == y || residual == y) {
-        set_error("moco_bn_add_relu_fwd_train: bad argument (null / misaligned pointer, in-place, eps <= 0, "
-                  "one of running_mean / running_var)");
-        return MOCO_ERR_INVALID;
-    }
-    if (workspace_bytes < bn_workspace_bytes()) { set_error("moco_bn_add_relu_fwd_train: workspace too small"); return MOCO_ERR_WORKSPACE; }
-    cudaError_t e = launch_bn_add_relu_fwd(x, residual, y, mask, M, C, *bn, shortcut, workspace,
-                                           static_cast<cudaStream_t>(stream_));
-    if (e == cudaErrorNotSupported) {
-        set_error("moco_bn_add_relu_fwd_train: needs M >= 1 and C a power of two in [64, 2048] (M=%lld C=%d)", M, C);
-        return MOCO_ERR_UNSUPPORTED;
-    }
-    if (e != cudaSuccess) return cuda_fail("batch-norm forward kernels", e);
-    return MOCO_OK;
+    if (!ptr16(x) || !ptr16(residual) || !ptr16(y) || !ptr16(workspace) || !bn_layer_fwd_ok(bn) ||
+        (shortcut && !bn_layer_fwd_ok(shortcut)) || x == y || residual == y)
+        return bn_bad_argument("moco_bn_add_relu_fwd_train", "null / misaligned pointer, in-place, eps <= 0, one of "
+                               "running_mean / running_var");
+    BnFwdPlan f{};
+    f.x = x; f.res = residual; f.y = y; f.mask = mask; f.ws = workspace; f.bn = bn; f.sc = shortcut;
+    f.M = M; f.C = C; f.relu = 1;
+    return bn_launch("moco_bn_add_relu_fwd_train", launch_bn_fwd, f, true, workspace_bytes, stream_);
 }
 
 int moco_bn_fwd_train_given(const void* x, const void* residual, void* y, void* mask, long long M, int C, int relu,
@@ -617,26 +624,16 @@ int moco_bn_fwd_train_given(const void* x, const void* residual, void* y, void* 
                             size_t workspace_bytes, void* stream_) {
     g_err[0] = 0;
     const bool passes = !(stats_given & MOCO_BN_STATS_GIVEN) || (shortcut && !(stats_given & MOCO_BN_SC_STATS_GIVEN));
-    if (!x || !y || !bn_layer_fwd_ok(bn) || (shortcut && (!bn_layer_fwd_ok(shortcut) || !residual)) ||
-        (stats_given & ~(MOCO_BN_STATS_GIVEN | MOCO_BN_SC_STATS_GIVEN)) || (passes && !workspace) || misaligned16(x) ||
-        misaligned16(residual) || misaligned16(y) || misaligned16(workspace) || x == y || residual == y) {
-        set_error("moco_bn_fwd_train_given: bad argument (null / misaligned pointer, in-place, eps <= 0, one of "
-                  "running_mean / running_var, unknown stats_given bits; a shortcut BN needs residual, a statistics "
-                  "pass the workspace)");
-        return MOCO_ERR_INVALID;
-    }
-    if (passes && workspace_bytes < bn_workspace_bytes()) {
-        set_error("moco_bn_fwd_train_given: workspace too small");
-        return MOCO_ERR_WORKSPACE;
-    }
-    cudaError_t e = launch_bn_fwd_given(x, residual, y, mask, M, C, relu, *bn, shortcut, stats_given, workspace,
-                                        static_cast<cudaStream_t>(stream_));
-    if (e == cudaErrorNotSupported) {
-        set_error("moco_bn_fwd_train_given: needs M >= 1 and C a power of two in [64, 2048] (M=%lld C=%d)", M, C);
-        return MOCO_ERR_UNSUPPORTED;
-    }
-    if (e != cudaSuccess) return cuda_fail("batch-norm forward kernels", e);
-    return MOCO_OK;
+    if (!ptr16(x) || !ptr16(y) || !bn_layer_fwd_ok(bn) || (shortcut && (!bn_layer_fwd_ok(shortcut) || !residual)) ||
+        (stats_given & ~(MOCO_BN_STATS_GIVEN | MOCO_BN_SC_STATS_GIVEN)) || (passes && !workspace) ||
+        misaligned16(residual) || misaligned16(workspace) || x == y || residual == y)
+        return bn_bad_argument("moco_bn_fwd_train_given", "null / misaligned pointer, in-place, eps <= 0, one of "
+                               "running_mean / running_var, unknown stats_given bits; a shortcut BN needs residual, a "
+                               "statistics pass the workspace");
+    BnFwdPlan f{};
+    f.x = x; f.res = residual; f.y = y; f.mask = mask; f.ws = workspace; f.bn = bn; f.sc = shortcut;
+    f.M = M; f.C = C; f.relu = relu; f.given = stats_given;
+    return bn_launch("moco_bn_fwd_train_given", launch_bn_fwd, f, passes, workspace_bytes, stream_);
 }
 
 size_t moco_conv1x1_workspace_bytes(void) { return conv1x1_workspace_bytes(); }
@@ -729,77 +726,52 @@ int moco_conv1x1_dgrad_bn_bwd(const void* dh, const void* w, void* g, long long 
 int moco_bn_bwd_apply_given(const void* g, const void* x, const void* x2, long long M, int C, const moco_bn_layer* bn,
                             const moco_bn_layer* shortcut, void* dx, void* dx2, void* stream_) {
     g_err[0] = 0;
-    if (!g || !x || !dx || !bn_layer_bwd_ok(bn) || (shortcut && (!bn_layer_bwd_ok(shortcut) || !x2 || !dx2)) ||
-        misaligned16(g) || misaligned16(x) || misaligned16(x2) || misaligned16(dx) || misaligned16(dx2)) {
-        set_error("moco_bn_bwd_apply_given: bad argument (null / misaligned pointer; x2 and dx2 are required with a "
-                  "shortcut BN)");
-        return MOCO_ERR_INVALID;
-    }
-    cudaError_t e = launch_bn_bwd_apply_given(g, x, x2, M, C, *bn, shortcut, dx, dx2,
-                                              static_cast<cudaStream_t>(stream_));
-    if (e == cudaErrorNotSupported) {
-        set_error("moco_bn_bwd_apply_given: needs M >= 1, C a power of two in [64, 2048] and no shortcut BN "
-                  "(M=%lld C=%d)", M, C);
-        return MOCO_ERR_UNSUPPORTED;
-    }
-    if (e != cudaSuccess) return cuda_fail("batch-norm backward kernels", e);
-    return MOCO_OK;
+    if (!ptr16(g) || !ptr16(x) || !ptr16(dx) || !bn_layer_bwd_ok(bn) ||
+        (shortcut && (!bn_layer_bwd_ok(shortcut) || !x2 || !dx2)) || misaligned16(x2) || misaligned16(dx2))
+        return bn_bad_argument("moco_bn_bwd_apply_given", "null / misaligned pointer; x2 and dx2 are required with a "
+                               "shortcut BN");
+    BnBwdPlan b{};
+    b.dy = g; b.x = x; b.x2 = x2; b.dx = dx; b.dres = dx2; b.bn = bn; b.sc = shortcut; b.M = M; b.C = C; b.reduced = 1;
+    return bn_launch("moco_bn_bwd_apply_given", launch_bn_bwd, b, false, 0, stream_);
+}
+
+// moco_bn_add_relu_bwd and (sum: dy2 is required) moco_bn_add_relu_bwd2
+static int bn_add_relu_bwd(const char* fn, bool sum, const void* dy, const void* dy2, const void* x,
+                           const void* residual, const void* mask, long long M, int C, const moco_bn_layer* bn,
+                           const moco_bn_layer* shortcut, void* dx, void* dresidual, void* workspace,
+                           size_t workspace_bytes, void* stream_) {
+    g_err[0] = 0;
+    if (!ptr16(dy) || (sum && !dy2) || !ptr16(x) || !mask || !ptr16(dx) || !ptr16(workspace) || !bn_layer_bwd_ok(bn) ||
+        (shortcut && (!bn_layer_bwd_ok(shortcut) || !residual || !dresidual)) || misaligned16(dy2) ||
+        misaligned16(residual) || misaligned16(dresidual))
+        return bn_bad_argument(fn, "null / misaligned pointer; residual and dresidual are required with a shortcut BN");
+    BnBwdPlan b{};
+    b.dy = dy; b.dy2 = dy2; b.x = x; b.mbits = mask; b.x2 = residual; b.dx = dx; b.dres = dresidual; b.ws = workspace;
+    b.bn = bn; b.sc = shortcut; b.M = M; b.C = C;
+    return bn_launch(fn, launch_bn_bwd, b, true, workspace_bytes, stream_);
 }
 
 int moco_bn_add_relu_bwd(const void* dy, const void* x, const void* residual, const void* mask, long long M, int C,
                          const moco_bn_layer* bn, const moco_bn_layer* shortcut, void* dx, void* dresidual,
                          void* workspace, size_t workspace_bytes, void* stream_) {
-    g_err[0] = 0;
-    if (!dy || !x || !mask || !dx || !workspace || !bn_layer_bwd_ok(bn) ||
-        (shortcut && (!bn_layer_bwd_ok(shortcut) || !residual || !dresidual)) || misaligned16(dy) || misaligned16(x) ||
-        misaligned16(residual) || misaligned16(dx) || misaligned16(dresidual) || misaligned16(workspace)) {
-        set_error("moco_bn_add_relu_bwd: bad argument (null / misaligned pointer; residual and dresidual are required "
-                  "with a shortcut BN)");
-        return MOCO_ERR_INVALID;
-    }
-    if (workspace_bytes < bn_workspace_bytes()) { set_error("moco_bn_add_relu_bwd: workspace too small"); return MOCO_ERR_WORKSPACE; }
-    cudaError_t e = launch_bn_add_relu_bwd(dy, nullptr, x, residual, mask, M, C, *bn, shortcut, dx, dresidual,
-                                           workspace, static_cast<cudaStream_t>(stream_));
-    if (e == cudaErrorNotSupported) {
-        set_error("moco_bn_add_relu_bwd: needs M >= 1 and C a power of two in [64, 2048] (M=%lld C=%d)", M, C);
-        return MOCO_ERR_UNSUPPORTED;
-    }
-    if (e != cudaSuccess) return cuda_fail("batch-norm backward kernels", e);
-    return MOCO_OK;
+    return bn_add_relu_bwd("moco_bn_add_relu_bwd", false, dy, nullptr, x, residual, mask, M, C, bn, shortcut, dx,
+                           dresidual, workspace, workspace_bytes, stream_);
 }
 
 int moco_bn_add_relu_bwd2(const void* dy, const void* dy2, const void* x, const void* residual, const void* mask,
                           long long M, int C, const moco_bn_layer* bn, const moco_bn_layer* shortcut, void* dx,
                           void* dresidual, void* workspace, size_t workspace_bytes, void* stream_) {
-    g_err[0] = 0;
-    if (!dy || !dy2 || !x || !mask || !dx || !workspace || !bn_layer_bwd_ok(bn) ||
-        (shortcut && (!bn_layer_bwd_ok(shortcut) || !residual || !dresidual)) || misaligned16(dy) ||
-        misaligned16(dy2) || misaligned16(x) || misaligned16(residual) || misaligned16(dx) || misaligned16(dresidual) ||
-        misaligned16(workspace)) {
-        set_error("moco_bn_add_relu_bwd2: bad argument (null / misaligned pointer; residual and dresidual are required "
-                  "with a shortcut BN)");
-        return MOCO_ERR_INVALID;
-    }
-    if (workspace_bytes < bn_workspace_bytes()) { set_error("moco_bn_add_relu_bwd2: workspace too small"); return MOCO_ERR_WORKSPACE; }
-    cudaError_t e = launch_bn_add_relu_bwd(dy, dy2, x, residual, mask, M, C, *bn, shortcut, dx, dresidual, workspace,
-                                           static_cast<cudaStream_t>(stream_));
-    if (e == cudaErrorNotSupported) {
-        set_error("moco_bn_add_relu_bwd2: needs M >= 1 and C a power of two in [64, 2048] (M=%lld C=%d)", M, C);
-        return MOCO_ERR_UNSUPPORTED;
-    }
-    if (e != cudaSuccess) return cuda_fail("batch-norm backward kernels", e);
-    return MOCO_OK;
+    return bn_add_relu_bwd("moco_bn_add_relu_bwd2", true, dy, dy2, x, residual, mask, M, C, bn, shortcut, dx,
+                           dresidual, workspace, workspace_bytes, stream_);
 }
 
 int moco_bn_relu_maxpool_fwd_train(const void* x, void* y, void* taps, int N, int H, int W, int C,
                                    const moco_bn_layer* bn, void* workspace, size_t workspace_bytes, void* stream_) {
     g_err[0] = 0;
-    if (!x || !y || !taps || !workspace || !bn_layer_fwd_ok(bn) || misaligned16(x) || misaligned16(y) ||
-        (reinterpret_cast<uintptr_t>(taps) & 7) || misaligned16(workspace)) {
-        set_error("moco_bn_relu_maxpool_fwd_train: bad argument (null / misaligned pointer, eps <= 0, "
-                  "one of running_mean / running_var)");
-        return MOCO_ERR_INVALID;
-    }
+    if (!ptr16(x) || !ptr16(y) || !taps || (reinterpret_cast<uintptr_t>(taps) & 7) || !ptr16(workspace) ||
+        !bn_layer_fwd_ok(bn))
+        return bn_bad_argument("moco_bn_relu_maxpool_fwd_train", "null / misaligned pointer, eps <= 0, one of "
+                               "running_mean / running_var");
     if (workspace_bytes < bn_workspace_bytes()) { set_error("moco_bn_relu_maxpool_fwd_train: workspace too small"); return MOCO_ERR_WORKSPACE; }
     cudaError_t e = launch_bn_relu_maxpool_fwd(x, y, taps, N, H, W, C, *bn, workspace, static_cast<cudaStream_t>(stream_));
     if (e == cudaErrorNotSupported) {

@@ -123,22 +123,26 @@ cudaError_t launch_maxpool_bwd(const void* dy, const void* dy2, const void* idx,
 cudaError_t launch_crop_to_s2d(const void* src, int src_dtype, long long img_stride, __nv_bfloat16* dst, int N, int H, int W,
                                cudaStream_t stream, const int64_t* src_rows);
 size_t bn_workspace_bytes();
-cudaError_t launch_bn_fwd_train(const void* x, const void* res, void* y, long long M, int C, const float* gamma,
-                                const float* beta, float* running_mean, float* running_var, long long* nbt, float momentum,
-                                float eps, int relu, float* save_mean, float* save_invstd, void* ws, cudaStream_t stream);
-cudaError_t launch_bn_bwd(const void* dy, const void* x, const void* y, long long M, int C, const float* gamma,
-                          const float* beta, const float* save_mean, const float* save_invstd, int relu, int has_residual,
-                          void* dx, void* dres, float* dgamma, float* dbeta, void* ws, cudaStream_t stream);
 using BnLayer = moco_bn_layer;
-cudaError_t launch_bn_add_relu_fwd(const void* x, const void* res, void* y, void* mask, long long M, int C,
-                                   const BnLayer& bn, const BnLayer* sc, void* ws, cudaStream_t stream);
-// given: MOCO_BN_STATS_GIVEN / MOCO_BN_SC_STATS_GIVEN, the layers whose save_mean / save_invstd are already final
-cudaError_t launch_bn_fwd_given(const void* x, const void* res, void* y, void* mask, long long M, int C, int relu,
-                                const BnLayer& bn, const BnLayer* sc, int given, void* ws, cudaStream_t stream);
-// dy2: nullable; a second gradient of y, added to dy (bf16 rounding of the sum) before the mask
-cudaError_t launch_bn_add_relu_bwd(const void* dy, const void* dy2, const void* x, const void* res, const void* mask,
-                                   long long M, int C, const BnLayer& bn, const BnLayer* sc, void* dx, void* dres,
-                                   void* ws, cudaStream_t stream);
+// a BatchNorm reduction's workspace: the slabs' ticket counters (zero between calls) at ws, then the per-CTA partials
+inline float* bn_ws_partials(void* ws) { return reinterpret_cast<float*>(static_cast<char*>(ws) + 256); }
+struct BnFwdPlan {              // the training forward: launch_bn_stats of each layer not `given`, then one apply pass
+    const void *x, *res;           // res: nullable; with sc the shortcut BN's input, added as bf16(sc(res))
+    void *y, *mask, *ws;           // mask: nullable, the ReLU mask bits of y for the backward; ws: unless all are given
+    const BnLayer *bn, *sc;        // sc: nullable, a downsample block's shortcut BN
+    long long M;
+    int C, relu, given;            // given: MOCO_BN_STATS_GIVEN | MOCO_BN_SC_STATS_GIVEN, whose save_* are final
+};
+cudaError_t launch_bn_fwd(const BnFwdPlan& f, cudaStream_t stream);
+struct BnBwdPlan {              // the training backward: the reduction pass (dbeta, dgamma), then the element-wise pass
+    const void *dy, *dy2, *x;      // dy2: nullable; a second gradient of y, added to dy (bf16 rounding of the sum)
+    const void *y, *mbits, *x2;    // the ReLU mask: the forward's bits, else y (has_residual) or x; x2: sc's input
+    void *dx, *dres, *ws;          // dres: the masked gradient (nullable), or with sc its input gradient (required)
+    const BnLayer *bn, *sc;
+    long long M;
+    int C, relu, has_residual, reduced;   // reduced: dy's sums are in bn->dbeta / dgamma, the element-wise pass alone
+};
+cudaError_t launch_bn_bwd(const BnBwdPlan& b, cudaStream_t stream);
 cudaError_t launch_bn_relu_maxpool_fwd(const void* x, void* y, void* taps, int N, int H, int W, int C, const BnLayer& bn,
                                        void* ws, cudaStream_t stream);
 cudaError_t launch_bn_eval_act(const void* x, const void* res, void* y, long long M, int C, const float* scale,
@@ -153,17 +157,12 @@ cudaError_t launch_bn_relu_maxpool_eval(const void* x, void* y, int N, int H, in
 void bn_stats_plan(long long M, int C, long long* passes, long long* ppc, int* R);
 // the same of the backward reduction pass (a multiple of kBnBwdReduceUnroll passes per CTA)
 void bn_bwd_reduce_plan(long long M, int C, long long* passes, long long* ppc, int* R);
-// the element-wise backward pass alone on an already-masked gradient g whose sums are in bn.dbeta / bn.dgamma (and
-// sc's): dx (and the shortcut BN's input gradient dx2)
-cudaError_t launch_bn_bwd_apply_given(const void* g, const void* x, const void* x2, long long M, int C, const BnLayer& bn,
-                                      const BnLayer* sc, void* dx, void* dx2, cudaStream_t stream);
 // the statistics pass alone (bn_stats_kernel): bn's save_mean / save_invstd and running statistics
 cudaError_t launch_bn_stats(const void* x, long long M, int C, const BnLayer& bn, void* ws, cudaStream_t stream);
 size_t conv1x1_workspace_bytes();
 cudaError_t launch_conv1x1_bn_stats(const void* x, const void* w, void* y, long long M, int Cin, int Cout,
                                     const BnLayer& bn, void* ws, cudaStream_t stream);
-// y = relu(bn(x . w^T) + r) recomputing the convolution (moco_conv1x1_bn_add_relu_fwd); given as for
-// launch_bn_fwd_given
+// y = relu(bn(x . w^T) + r) recomputing the convolution (moco_conv1x1_bn_add_relu_fwd); given as in BnFwdPlan
 cudaError_t launch_conv1x1_bn_add_relu(const void* x, const void* w, const void* res, void* y, void* mask, long long M,
                                        int Cin, int Cout, const BnLayer& bn, const BnLayer* sc, int given, void* ws,
                                        cudaStream_t stream);

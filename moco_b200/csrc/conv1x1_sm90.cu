@@ -270,7 +270,7 @@ static cudaError_t launch_bn(const void* x, const void* w, void* y, int M, int C
     const int smem = stages * S::kStage + S::kFixed + kBarBytes;
     a.momentum = bn.momentum; a.eps = bn.eps;
     a.counters = static_cast<unsigned int*>(ws);
-    a.partial = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 256);
+    a.partial = bn_ws_partials(ws);
     a.mean = bn.save_mean; a.invstd = bn.save_invstd;
     a.running_mean = bn.running_mean; a.running_var = bn.running_var; a.num_batches_tracked = bn.num_batches_tracked;
     a.store = y != nullptr;
@@ -782,7 +782,7 @@ cudaError_t launch_conv1x1_dgrad_bn_bwd(const void* dh, const void* w, void* g, 
     a.stages = stages;
     const int smem = stages * S::kStage + S::kFixed + kBarBytes;
     a.counters = static_cast<unsigned int*>(ws);
-    a.partial = reinterpret_cast<float*>(static_cast<uint8_t*>(ws) + 256);
+    a.partial = bn_ws_partials(ws);
     a.mean = bn.save_mean; a.invstd = bn.save_invstd; a.dgamma = bn.dgamma; a.dbeta = bn.dbeta;
     CUtensorMap tm_dh, tm_w, tm_x, tm_dy2, tm_mask, tm_g;
     if (!make_tmap(&tm_dh, dh, (int)M, Cout, kCvBM) || !make_tmap(&tm_w, w, Cout, Cin, 64) ||
