@@ -701,7 +701,7 @@ int moco_conv1x1_dgrad_bn_bwd(const void* dh, const void* w, void* g, long long 
     if (!dh || !w || !g || !x || !workspace || !bn || !bn->save_mean || !bn->save_invstd || !bn->dgamma ||
         !bn->dbeta || (x2 == nullptr) != (shortcut == nullptr) || misaligned16(dh) || misaligned16(w) ||
         misaligned16(g) || misaligned16(x) || misaligned16(mask) || misaligned16(dy2) || misaligned16(x2) ||
-        misaligned16(workspace) || g == dh || g == x || g == dy2) {
+        misaligned16(workspace) || g == dh || g == w || g == x || g == mask || g == dy2) {
         set_error("moco_conv1x1_dgrad_bn_bwd: bad argument (null / misaligned pointer, g aliasing an input, x2 without "
                   "the shortcut BN or the reverse)");
         return MOCO_ERR_INVALID;

@@ -32,30 +32,31 @@ CINS = [64, 192, 1088, 4096]                      # 1, 3, 17 and 64 K chunks
 SMALL_M = [1, 31, 32, 127, 128, 129, 255, 256, 257, 258]   # the 128-row tile and the 256-row statistics chunk
 
 
-def _plan(M, C):
-    """bn_reduce_plan (csrc/bn_nhwc.cu) as bn_stats_plan calls it (8 passes unrolled, 2 CTAs per SM, 132 SMs): the
-    passes of 32 rows, the passes of each CTA's row chunk and R, the CTAs per 64-channel slab."""
+def _plan(M, C, unroll=8):
+    """bn_reduce_plan (csrc/bn_nhwc.cu) with 2 CTAs per SM and kBnSms = 132, as bn_stats_plan calls it (unroll 8) or
+    bn_bwd_reduce_plan (unroll 4): the passes of 32 rows, the passes of each CTA's row chunk and R, the CTAs per
+    64-channel slab."""
     passes = -(-M // 32)
-    r = max(1, min(132 * 2 // (C // 64), -(-passes // 8)))
+    r = max(1, min(132 * 2 // (C // 64), -(-passes // unroll)))
     per = -(-passes // r)
-    per = -(-per // 8) * 8
+    per = -(-per // unroll) * unroll
     return passes, per, -(-passes // per)
 
 
-def _r_changes(C, limit):
+def _r_changes(C, limit, unroll=8):
     """The row counts M <= limit at which the plan's R differs from its value at M - 1 (M = 1 first)."""
     out, prev = [], None
     for p in range(1, -(-limit // 32) + 1):
-        R = _plan(32 * p, C)[2]
+        R = _plan(32 * p, C, unroll)[2]
         if R != prev:
             out.append(32 * p - 31)
             prev = R
     return out
 
 
-def _planted(M, C):
+def _planted(M, C, unroll=8):
     """The planted rows of an M-row case with C channels (row 0 excluded: it holds the shift)."""
-    _, per, R = _plan(M, C)
+    _, per, R = _plan(M, C, unroll)
     L = 32 * per
     rows = set()
     for k in range(R):

@@ -22,6 +22,7 @@ def test_conv1x1_dgrad_bn_bwd_validates_its_arguments():
     for bad in [dict(dh=None), dict(w=None), dict(g=None), dict(x=None), dict(work=None), dict(layer=_layer(None)),
                 dict(dh=FAKE + 8), dict(w=FAKE + 2), dict(g=FAKE + 4), dict(x=FAKE + 8), dict(mask=FAKE + 1),
                 dict(dy2=FAKE + 8), dict(work=FAKE + 8), dict(g=FAKE), dict(g=FAKE + 12288), dict(g=FAKE + 20480),
+                dict(g=FAKE + 4096), dict(g=FAKE + 16384),           # g aliasing w or the mask bytes
                 dict(x2=FAKE + 28672),                               # x2 without the shortcut BN
                 dict(sc=_layer())]:                                  # and the reverse
         assert call(**bad) == -1, bad
