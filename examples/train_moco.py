@@ -8,6 +8,7 @@ Launch compatibility (SURVEY.md §8b): the reference only understands ``--local_
 (``$LOCAL_RANK``).  This entry point accepts all three:
 
     python examples/train_moco.py --steps 20                                            # 1 GPU
+    python examples/train_moco.py --data-dir /data/imagenet --steps 20                  # real images (train/)
     torchrun --nproc-per-node 8 --master-addr 127.0.0.1 examples/train_moco.py --steps 20
 """
 import argparse
@@ -35,7 +36,25 @@ def parse_args(argv=None):
                     help="encoders return the raw fc output; L2 normalisation (resnet.py:24-33) runs inside the head kernels")
     ap.add_argument("--graph-tail", action="store_true",
                     help="single GPU: replay everything after the key encoder from one CUDA graph (device-side ring index)")
+    ap.add_argument("--data-dir", default="",
+                    help="ImageFolder root with train/ (train.py:94); decoded by the workers, augmented on the GPU "
+                         "(moco_b200/augment.py).  Without it the inputs are synthetic.")
+    ap.add_argument("--crop", type=float, default=0.08, help="minimum crop scale (train.py: --crop)")
+    ap.add_argument("--aug", default="CJ", choices=["NULL", "CJ"], help="train.py: --aug")
+    ap.add_argument("--num-workers", type=int, default=4, help="DataLoader workers per GPU (train.py: --num-workers)")
     return ap.parse_args(argv)
+
+
+def make_loader(args, world):
+    """train.py:92-125 with the pixel work moved to the GPU: the workers decode and draw the crop parameters only."""
+    import torch
+    from moco_b200.augment import ImageFolderTwoCrop
+    dataset = ImageFolderTwoCrop(os.path.join(args.data_dir, "train"), scale=(args.crop, 1.0), aug=args.aug)
+    sampler = torch.utils.data.distributed.DistributedSampler(dataset, drop_last=True) if world > 1 else None
+    return torch.utils.data.DataLoader(dataset, batch_size=args.batch_size, shuffle=sampler is None,
+                                       num_workers=args.num_workers, pin_memory=True, sampler=sampler,
+                                       drop_last=True, collate_fn=ImageFolderTwoCrop.collate_fn,
+                                       persistent_workers=args.num_workers > 0)
 
 
 def main(argv=None):
@@ -78,8 +97,16 @@ def main(argv=None):
                     fuse_normalize=args.fuse_normalize, graph_tail=args.graph_tail)
 
     gen = torch.Generator(device=dev).manual_seed(1234 + rank)
+    batches = None
+    if args.data_dir:
+        from moco_b200.augment import augment_two_crop
+        loader = make_loader(args, world)
+        batches = _cycle(loader)
     for it in range(args.steps):
-        inputs = torch.randn(args.batch_size, 6, 224, 224, device=dev, generator=gen)    # dataset.py:31-33 layout
+        if batches is not None:
+            inputs = augment_two_crop(next(batches))                                     # replaces train.py:253-254
+        else:
+            inputs = torch.randn(args.batch_size, 6, 224, 224, device=dev, generator=gen)    # dataset.py:31-33 layout
         x1, x2 = torch.split(inputs, [3, 3], dim=1)                                      # train.py:250
         loss, prob = step(x1, x2, args.epoch)
         if rank == 0 and (it % 10 == 0 or it == args.steps - 1):
@@ -91,6 +118,15 @@ def main(argv=None):
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
+
+
+def _cycle(loader):
+    epoch = 0
+    while True:
+        if getattr(loader, "sampler", None) is not None and hasattr(loader.sampler, "set_epoch"):
+            loader.sampler.set_epoch(epoch)                                              # train.py:213
+        yield from loader
+        epoch += 1
 
 
 if __name__ == "__main__":

@@ -506,6 +506,48 @@ int moco_crop_gather_nhwc_bf16(const void* src, int src_dtype, long long src_ima
                                void* dst_bf16, int N, int C, int HW, void* stream);
 
 /* ------------------------------------------------------------------------
+ * Data augmentation of the two pre-training crops (train.py:106-114 applied twice per image, moco/dataset.py:25-33)
+ * from decoded uint8 images: the loader's workers only decode and draw the random parameters, and the device receives
+ * the source pixels instead of fp32 [N, 6, 224, 224] crops.
+ *
+ * Crop i is torchvision's TENSOR implementation (torchvision.transforms.functional) of the reference's transform,
+ * applied to x = src_uint8 / 255 in fp32, with the parameters of record crops[i]:
+ *   1. resized_crop(x, top, left, height, width, [out_h, out_w], antialias=True): ATen's upsample_bilinear2d_aa,
+ *      triangle filter of support max(scale, 1), taps clipped at the crop's border, weights renormalised;
+ *   2. rgb_to_grayscale(x, 3) (0.2989 r + 0.587 g + 0.114 b) when flags has MOCO_AUG_GRAY;
+ *   3. when flags has MOCO_AUG_JITTER, for k = 0..3 op (order >> 2k) & 3 (ColorJitter's fn_idx):
+ *      0 adjust_brightness, 1 adjust_contrast, 2 adjust_saturation, 3 adjust_hue with the record's factors;
+ *      _blend(a, b, r) = clamp(r a + (1 - r) b, 0, 1); the contrast mean is the mean grayscale of the whole crop as it
+ *      stands before the contrast op; hue via _rgb2hsv / _hsv2rgb with the shifted hue taken % 1.0;
+ *   4. hflip when flags has MOCO_AUG_FLIP;
+ *   5. (x - mean[c]) / std[c], a subtraction then a division (norm_host = {mean[3], std[3]}, a HOST array).
+ * Every step is fp32 in torchvision's operation order; the resample's sums are ordered differently from ATen's CPU
+ * kernel (vertical pass first), so results agree with torchvision to fp32 rounding, not bit for bit.  The
+ * reference itself runs PIL on uint8, which rounds after every step: this is the documented deviation from it.
+ *
+ * pixels: packed uint8 HWC RGB images, image of crop i at byte crops[i].src_offset (src_h * src_w * 3 bytes).
+ * crops: DEVICE array of n_crops records.  dst: crop i at dst + i * 3 * out_h * out_w elements, three NCHW planes,
+ * MOCO_F32 or MOCO_BF16 (the round-to-nearest-even of the fp32 value): a [2N, 3, H, W] tensor of crops
+ * (2n, 2n + 1) of image n is the reference's [N, 6, H, W] batch.  crop_means: DEVICE float [n_crops] scratch (the
+ * contrast means).  out_h, out_w in [1, 1024]; n_crops in [0, 65535]; a crop at most 1000 * out_w pixels wide.
+ * The records are validated on the host by the caller (moco_b200/augment.py); here every source index is clamped
+ * into its own image and into [0, pixels_bytes), so a malformed record gives unspecified values but never reads
+ * outside the buffer.  Two launches (the contrast means, then the crops); deterministic.
+ * ---------------------------------------------------------------------- */
+enum { MOCO_AUG_GRAY = 1, MOCO_AUG_FLIP = 2, MOCO_AUG_JITTER = 4 };
+typedef struct moco_aug_crop {
+    int64_t src_offset;                   /* byte offset of the source image in `pixels`                 */
+    int32_t src_h, src_w;                 /* source image size                                           */
+    int32_t top, left, height, width;     /* crop box (RandomResizedCrop.get_params: i, j, h, w)         */
+    int32_t flags;                        /* MOCO_AUG_*                                                  */
+    int32_t order;                        /* ColorJitter's fn_idx, op k in bits 2k..2k+1                 */
+    float brightness, contrast, saturation, hue;
+} moco_aug_crop;                          /* 56 bytes                                                    */
+
+int moco_augment_crops(const void* pixels, size_t pixels_bytes, const moco_aug_crop* crops, int n_crops, int out_h,
+                       int out_w, const float* norm_host, void* dst, int dst_dtype, float* crop_means, void* stream);
+
+/* ------------------------------------------------------------------------
  * ShuffleBN row gather over NVLink peer memory.  Replaces dist_collect +
  * fancy-index (moco/util.py:47-58,74-79,88-91): instead of all_gather-ing every
  * rank's batch and indexing, each rank pulls exactly the rows it needs.

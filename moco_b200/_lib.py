@@ -19,6 +19,7 @@ NCE_TWO_PASS, NCE_ONE_PASS = 512, 1024
 ONE_PASS_MAX_INV_T = 25.0          # MOCO_ONE_PASS_MAX_INV_T (include/moco_b200.h)
 GATHER_AUTO, GATHER_LDG = 0, 1
 BN_STATS_GIVEN, BN_SC_STATS_GIVEN = 1, 2    # moco_bn_fwd_train_given `stats_given` bits
+AUG_GRAY, AUG_FLIP, AUG_JITTER = 1, 2, 4    # moco_aug_crop `flags` bits
 
 
 
@@ -96,6 +97,8 @@ SIGNATURES = {
     "moco_bn_relu_maxpool_eval": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "moco_bn_eval_act_avgpool": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
                                          c_void_p, c_void_p, c_void_p]),
+    "moco_augment_crops": (c_int, [c_void_p, c_size_t, c_void_p, c_int, c_int, c_int, POINTER(c_float), c_void_p, c_int,
+                                   c_void_p, c_void_p]),
     "moco_crop_to_nhwc_bf16": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_int, c_int, c_void_p]),
     "moco_shuffle_gather": (c_int, [POINTER(c_void_p), c_int, c_int, c_void_p, c_int, c_size_t, c_void_p, c_int, c_void_p]),
     "moco_shuffle_gather_sync": (c_int, [POINTER(c_void_p), POINTER(c_void_p), c_int, c_int, c_uint32, c_int, c_void_p, c_int,
@@ -151,6 +154,7 @@ class _Counting:
     _PER_CALL = {"moco_nce_shard_stats": 3, "moco_nce_shard_merge": 1, "moco_nce_shard_dq": 2,
                  "moco_nce_shard_dq_finish": 1, "moco_nce_shard_dq_finish_peers": 1, "moco_queue_enqueue_shard": 1, "moco_queue_enqueue": 1, "moco_f32_to_bf16": 1, "moco_shuffle_gather": 1, "moco_shuffle_gather_sync": 1, "moco_crop_gather_nhwc_bf16": 1,
                  "moco_ema_update": 1, "moco_crop_to_nhwc_bf16": 1, "moco_bn_fwd_train": 2, "moco_bn_bwd": 2, "moco_bn_add_relu_bwd": 2, "moco_bn_add_relu_bwd2": 2, "moco_bn_relu_maxpool_fwd_train": 2, "moco_bn_eval_act": 1, "moco_bn_relu_maxpool_eval": 1, "moco_bn_eval_act_avgpool": 1, "moco_crop_s2d_bf16": 1, "moco_conv1x1_bn_stats": 1, "moco_conv1x1_dgrad_bn_bwd": 1, "moco_bn_bwd_apply_given": 1, "moco_maxpool3x3s2_fwd": 1, "moco_maxpool3x3s2_bwd": 1, "moco_maxpool3x3s2_bwd2": 1,
+                 "moco_augment_crops": 2,
                  "moco_signal_barrier": 1, "moco_nce_bwd_dense": 1}
 
     def __init__(self, lib):

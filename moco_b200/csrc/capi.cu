@@ -524,6 +524,35 @@ int moco_crop_s2d_bf16(const void* src, int src_dtype, long long src_image_strid
     return MOCO_OK;
 }
 
+int moco_augment_crops(const void* pixels, size_t pixels_bytes, const moco_aug_crop* crops, int n_crops, int out_h,
+                       int out_w, const float* norm, void* dst, int dst_dtype, float* crop_means, void* stream_) {
+    g_err[0] = 0;
+    static_assert(sizeof(moco_aug_crop) == 56, "moco_aug_crop is 14 32-bit words ([2N, 14] int32 on the host side)");
+    if (!norm || (dst_dtype != MOCO_F32 && dst_dtype != MOCO_BF16) ||
+        (n_crops > 0 && (!pixels || pixels_bytes == 0 || !crops || !dst || !crop_means ||
+                         (reinterpret_cast<uintptr_t>(crops) & 7) || (reinterpret_cast<uintptr_t>(crop_means) & 3) ||
+                         (reinterpret_cast<uintptr_t>(dst) & (dst_dtype == MOCO_F32 ? 3 : 1))))) {
+        set_error("moco_augment_crops: bad argument (null or misaligned pointer, empty pixel buffer, or dst_dtype=%d)",
+                  dst_dtype);
+        return MOCO_ERR_INVALID;
+    }
+    for (int k = 0; k < 6; ++k) {
+        if (!isfinite(norm[k]) || (k >= 3 && norm[k] == 0.f)) {
+            set_error("moco_augment_crops: norm must be finite mean[3], std[3] with std != 0");
+            return MOCO_ERR_INVALID;
+        }
+    }
+    if (!augment_shape_ok(n_crops, out_h, out_w)) {
+        set_error("moco_augment_crops: needs n_crops in [0, 65535] and out_h, out_w in [1, 1024] (n_crops=%d out_h=%d "
+                  "out_w=%d)", n_crops, out_h, out_w);
+        return MOCO_ERR_INVALID;
+    }
+    cudaError_t e = launch_augment(pixels, pixels_bytes, crops, n_crops, out_h, out_w, norm, dst, dst_dtype, crop_means,
+                                   static_cast<cudaStream_t>(stream_));
+    if (e != cudaSuccess) return cuda_fail("augment kernels", e);
+    return MOCO_OK;
+}
+
 int moco_maxpool3x3s2_fwd(const void* x, void* y, void* taps, int N, int H, int W, int C, void* stream_) {
     g_err[0] = 0;
     if (!x || !y || !taps || (reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(y) & 15) ||

@@ -171,6 +171,10 @@ cudaError_t launch_conv1x1_bn_add_relu(const void* x, const void* w, const void*
 cudaError_t launch_conv1x1_dgrad_bn_bwd(const void* dh, const void* w, void* g, long long M, int Cin, int Cout,
                                         const void* x, const void* mask, const void* dy2, const BnLayer& bn, void* ws,
                                         cudaStream_t stream);
+bool augment_shape_ok(int n_crops, int out_h, int out_w);
+cudaError_t launch_augment(const void* pixels, size_t pixels_bytes, const moco_aug_crop* crops, int n_crops, int out_h,
+                           int out_w, const float norm[6], void* dst, int dst_dtype, float* crop_means,
+                           cudaStream_t stream);
 int ema_chunk_elems();
 cudaError_t launch_ema(const void* segs, const int* chunk_prefix, int n_segs, int n_chunks, float m,
                        float one_minus_m, cudaStream_t stream);
