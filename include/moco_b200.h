@@ -12,7 +12,8 @@
  *   - every pointer is a DEVICE pointer unless the name ends in `_host`;
  *   - compute calls are asynchronous on `stream` (a cudaStream_t passed as
  *     void*), re-entrant, allocate nothing and keep no global state besides the
- *     cached cuTensorMapEncodeTiled entry point; they are CUDA-graph capturable;
+ *     cached cuTensorMapEncodeTiled entry point and the launch counter
+ *     (moco_launch_count); they are CUDA-graph capturable;
  *   - return value: 0 on success, a negative MOCO_ERR_* otherwise;
  *     moco_last_error() returns a thread-local human readable message;
  *   - row-major everywhere; `queue` is the [K, C] MoCo memory bank.
@@ -27,7 +28,8 @@
 extern "C" {
 #endif
 
-#define MOCO_B200_ABI_VERSION 3 /* 3: + moco_bn_*, moco_maxpool3x3s2_*, moco_crop_s2d_bf16, moco_conv1x1_* (additive) */
+#define MOCO_B200_ABI_VERSION 3 /* 3: + moco_bn_*, moco_maxpool3x3s2_*, moco_crop_s2d_bf16, moco_conv1x1_*,
+                                    moco_augment_crops, moco_launch_count (additive) */
 
 enum {
     MOCO_OK = 0,
@@ -65,6 +67,11 @@ const char* moco_last_error(void);
 
 /* Number of SMs / compute capability of the current device (for tests & bench). */
 int moco_device_info(int* sm_count, int* cc_major, int* cc_minor);
+
+/* Kernels this library has launched in this process, on all devices and threads: every kernel whose launch call
+ * succeeded.  A launch recorded during stream capture counts once, when it is captured; replays of the graph do not
+ * count. */
+unsigned long long moco_launch_count(void);
 
 /* ------------------------------------------------------------------------
  * InfoNCE head:  MemoryMoCo.forward logits (moco/NCE/Contrast.py:20-27) fused

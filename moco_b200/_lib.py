@@ -3,12 +3,15 @@
 The library is built in-tree by ``moco_b200/build.py`` (nvcc, sm_90a).  There is
 no CPU fallback: if the shared object is missing and cannot be built, importing
 any compute entry point raises.
+
+``load()`` returns the ``ctypes.CDLL`` itself.  ``launches`` reads ``moco_launch_count()``: the kernels the library
+has launched in this process, counted in C where each kernel is launched.
 """
 from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, c_char_p, c_float, c_int, c_int64, c_size_t, c_uint32, c_void_p
+from ctypes import POINTER, c_char_p, c_float, c_int, c_int64, c_size_t, c_uint32, c_ulonglong, c_void_p
 
 from . import build as _build
 
@@ -35,6 +38,7 @@ SIGNATURES = {
     "moco_abi_version": (c_int, []),
     "moco_last_error": (c_char_p, []),
     "moco_device_info": (c_int, [POINTER(c_int), POINTER(c_int), POINTER(c_int)]),
+    "moco_launch_count": (c_ulonglong, []),
     "moco_nce_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "moco_nce_fwd": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_int, c_int, c_int, c_float,
                              c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -140,115 +144,14 @@ def load() -> ctypes.CDLL:
         fn.argtypes = args
     if lib.moco_abi_version() != ABI_VERSION:
         raise RuntimeError("moco_b200: ABI version mismatch between _lib.py and libmoco_b200.so")
-    _lib = _Counting(lib)
+    _lib = lib
     return _lib
 
 
-# kernels launched per successful C-ABI call (bench.py reports the total as `gpu_launches`)
-launches = 0
-
-
-class _Counting:
-    """Thin proxy over the CDLL that counts this library's kernel launches."""
-
-    _PER_CALL = {"moco_nce_shard_stats": 3, "moco_nce_shard_merge": 1, "moco_nce_shard_dq": 2,
-                 "moco_nce_shard_dq_finish": 1, "moco_nce_shard_dq_finish_peers": 1, "moco_queue_enqueue_shard": 1, "moco_queue_enqueue": 1, "moco_f32_to_bf16": 1, "moco_shuffle_gather": 1, "moco_shuffle_gather_sync": 1, "moco_crop_gather_nhwc_bf16": 1,
-                 "moco_ema_update": 1, "moco_crop_to_nhwc_bf16": 1, "moco_bn_fwd_train": 2, "moco_bn_bwd": 2, "moco_bn_add_relu_bwd": 2, "moco_bn_add_relu_bwd2": 2, "moco_bn_relu_maxpool_fwd_train": 2, "moco_bn_eval_act": 1, "moco_bn_relu_maxpool_eval": 1, "moco_bn_eval_act_avgpool": 1, "moco_crop_s2d_bf16": 1, "moco_conv1x1_bn_stats": 1, "moco_conv1x1_dgrad_bn_bwd": 1, "moco_bn_bwd_apply_given": 1, "moco_maxpool3x3s2_fwd": 1, "moco_maxpool3x3s2_bwd": 1, "moco_maxpool3x3s2_bwd2": 1,
-                 "moco_augment_crops": 2,
-                 "moco_signal_barrier": 1, "moco_nce_bwd_dense": 1}
-
-    def __init__(self, lib):
-        self._lib = lib
-        for name in SIGNATURES:
-            fn = getattr(lib, name)
-            if name == "moco_nce_fwd":
-                setattr(self, name, self._wrap_nce(fn))
-            elif name == "moco_nce_step":
-                setattr(self, name, self._wrap_step(fn))
-            elif name == "moco_nce_shard_dq":      # one-pass finish: dq_reduce only; two-pass: dq kernel + dq_reduce
-                setattr(self, name, self._wrap_flags(fn, 11))
-            elif name == "moco_bn_add_relu_fwd_train":  # + the shortcut BN's statistics pass
-                setattr(self, name, self._wrap_count(fn, lambda a: 3 if a[7] is not None else 2))
-            elif name == "moco_bn_fwd_train_given":     # the apply pass + the statistics passes not given
-                setattr(self, name, self._wrap_count(fn, lambda a: 1 + (not a[9] & BN_STATS_GIVEN)
-                                                     + (a[8] is not None and not a[9] & BN_SC_STATS_GIVEN)))
-            elif name == "moco_conv1x1_bn_add_relu_fwd":  # the same, with the GEMM's statistics pass
-                setattr(self, name, self._wrap_count(fn, lambda a: 1 + (not a[10] & BN_STATS_GIVEN)
-                                                     + (a[9] is not None and not a[10] & BN_SC_STATS_GIVEN)))
-            elif name in self._PER_CALL:
-                setattr(self, name, self._wrap(fn, self._PER_CALL[name]))
-            else:
-                setattr(self, name, fn)
-
-    @staticmethod
-    def _wrap(fn, n):
-        def call(*a):
-            global launches
-            rc = fn(*a)
-            if rc == 0:
-                launches += n
-            return rc
-        return call
-
-    @staticmethod
-    def _wrap_count(fn, count):
-        def call(*a):
-            global launches
-            rc = fn(*a)
-            if rc == 0:
-                launches += count(a)
-            return rc
-        return call
-
-    @staticmethod
-    def _wrap_flags(fn, flag_index):
-        def call(*a):
-            global launches
-            rc = fn(*a)
-            if rc == 0:
-                launches += 1 if (a[flag_index] & NCE_ONE_PASS) else 2
-            return rc
-        return call
-
-    def _sm_count(self):
-        sms = c_int(0)
-        return sms.value if self._lib.moco_device_info(ctypes.byref(sms), None, None) == 0 else 0
-
-    @staticmethod
-    def _head_plan(N, C, inv_T, flags, dq, logits, f32, sms):
-        """(kernels one head evaluation launches, whether it took the one-sweep path): mirrors the dispatch in
-        csrc/capi.cu.  The tensor-core kernels put one 128-row block of q on each SM, so beyond 128 * #SM rows
-        every flag ends on the CUDA-core kernel."""
-        tc = not (flags & NCE_FORCE_SIMT) and C % 64 == 0 and C <= 256 and (N + 127) // 128 <= sms
-        if not tc:
-            return 2, False                                      # prep + row kernel
-        one_pass = (dq and not logits and not (flags & NCE_TWO_PASS)
-                    and ((flags & NCE_ONE_PASS) or inv_T <= ONE_PASS_MAX_INV_T))
-        if one_pass:                                             # sweep + tail (+ prep for the bf16 copy at C > 128)
-            return 2 + (1 if (C > 128 and f32) else 0), True
-        return (5 if dq else 3), False                           # prep + stats + combine [+ dq + dq_reduce]
-
-    def _wrap_nce(self, fn):
-        def call(*a):
-            global launches
-            rc = fn(*a)
-            if rc == 0:
-                launches += self._head_plan(a[4], a[5], a[7], a[16], a[13], a[8], a[2] == MOCO_F32, self._sm_count())[0]
-            return rc
-        return call
-
-    def _wrap_step(self, fn):
-        def call(*a):
-            global launches
-            rc = fn(*a)
-            if rc == 0:
-                C = a[7]
-                n, one_pass = self._head_plan(a[6], C, a[9], a[22], a[19] is not None, False, a[2] == MOCO_F32,
-                                              self._sm_count())
-                fused = one_pass and C % 8 == 0 and 256 % (C // 8) == 0      # the tail kernel also enqueues
-                launches += n + (0 if (fused or a[12] == 0) else 1)
-            return rc
-        return call
+def __getattr__(name):
+    if name == "launches":             # bench.py reports the delta over its timed steps as `gpu_launches`
+        return load().moco_launch_count()
+    raise AttributeError(f"module {__name__!r} has no attribute {name!r}")
 
 
 def check(code: int, what: str) -> None:

@@ -304,10 +304,10 @@ cudaError_t launch_augment(const void* pixels, size_t pixels_bytes, const moco_a
     p.dtype = dst_dtype;
     p.means = crop_means;
     aug_mean_kernel<<<n_crops, kAugThreads, 0, stream>>>(p);
-    cudaError_t e = cudaGetLastError();
+    cudaError_t e = launched();
     if (e != cudaSuccess) return e;
     aug_apply_kernel<<<dim3((out_h + kAugRows - 1) / kAugRows, n_crops), kAugThreads, 0, stream>>>(p);
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace moco

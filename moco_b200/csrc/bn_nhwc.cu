@@ -590,23 +590,23 @@ template <int U, int CT>
 static cudaError_t run_stats(BnStatsArgs& s, cudaStream_t stream) {
     bn_reduce_plan(s.M, s.C, U, CT, &s.passes, &s.ppc, &s.R);
     bn_stats_kernel<U, CT><<<dim3(s.C / kBnSlab, s.R), kBnThreads, 0, stream>>>(s);
-    return cudaGetLastError();
+    return launched();
 }
 template <int U, int CT, bool SC>
 static cudaError_t run_apply(BnApplyArgs& p, cudaStream_t stream) {
     bn_apply_kernel<U, CT, SC><<<bn_apply_grid(p.V, U, CT), kBnThreads, 0, stream>>>(p);
-    return cudaGetLastError();
+    return launched();
 }
 template <int U, int CT, bool SC, bool SUM = false>
 static cudaError_t run_bwd_reduce(BnBwdReduceArgs& s, cudaStream_t stream) {
     bn_reduce_plan(s.M, s.C, U, CT, &s.passes, &s.ppc, &s.R);
     bn_bwd_reduce_kernel<U, CT, SC, SUM><<<dim3(s.C / kBnSlab, s.R), kBnThreads, 0, stream>>>(s);
-    return cudaGetLastError();
+    return launched();
 }
 template <int U, int CT, bool SC, bool SUM = false>
 static cudaError_t run_bwd_apply(BnBwdApplyArgs& p, cudaStream_t stream) {
     bn_bwd_apply_kernel<U, CT, SC, SUM><<<bn_apply_grid(p.V, U, CT), kBnThreads, 0, stream>>>(p);
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t launch_bn_stats(const void* x, long long M, int C, const BnLayer& bn, void* ws, cudaStream_t stream) {
@@ -713,7 +713,7 @@ cudaError_t launch_bn_eval_act(const void* x, const void* res, void* y, long lon
     const int grid = bn_apply_grid(a.V, kBnApplyUnroll, kBnApplyCtas);
     if (sc_scale != nullptr) bn_eval_kernel<true><<<grid, kBnThreads, 0, stream>>>(a);
     else bn_eval_kernel<false><<<grid, kBnThreads, 0, stream>>>(a);
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t launch_bn_eval_act_avgpool(const void* x, const void* res, float* feat, int N, int HW, int C,
@@ -728,7 +728,7 @@ cudaError_t launch_bn_eval_act_avgpool(const void* x, const void* res, float* fe
     if (blocks > 0x7fffffffLL) return cudaErrorNotSupported;
     if (sc_scale != nullptr) bn_eval_avgpool_kernel<true><<<(unsigned int)blocks, kBnPoolThreads, 0, stream>>>(a);
     else bn_eval_avgpool_kernel<false><<<(unsigned int)blocks, kBnPoolThreads, 0, stream>>>(a);
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t launch_bn_relu_maxpool_eval(const void* x, void* y, int N, int H, int W, int C, const float* scale,

@@ -9,6 +9,7 @@
 namespace moco {
 
 static thread_local char g_err[512] = "";
+std::atomic<unsigned long long> g_launch_count{0};
 
 void set_error(const char* fmt, ...) {
     va_list ap;
@@ -96,6 +97,8 @@ int moco_device_info(int* sm_count, int* cc_major, int* cc_minor) {
     if (cc_minor) *cc_minor = d.minor;
     return MOCO_OK;
 }
+
+unsigned long long moco_launch_count(void) { return g_launch_count.load(std::memory_order_relaxed); }
 
 size_t moco_nce_workspace_bytes(int N, int C, int K) {
     (void)K;

@@ -6,6 +6,8 @@
 #include <stdint.h>
 #include <stdlib.h>
 
+#include <atomic>
+
 #include "../../include/moco_b200.h"
 
 namespace moco {
@@ -39,6 +41,15 @@ struct ShardExact {
     float inv_T;
 };
 
+// The kernels launched in this process (moco_launch_count).  Every launch of the library passes its result through
+// counted(): launch_pdl and launch_cluster wrap cudaLaunchKernelEx in it, and each <<<...>>> is followed by launched().
+extern std::atomic<unsigned long long> g_launch_count;
+inline cudaError_t counted(cudaError_t e) {
+    if (e == cudaSuccess) g_launch_count.fetch_add(1, std::memory_order_relaxed);
+    return e;
+}
+inline cudaError_t launched() { return counted(cudaGetLastError()); }
+
 // Programmatic dependent launch for the head's kernel chain (prep -> one-pass | stats -> combine [-> dq] -> dq_reduce
 // -> enqueue): at MoCo's default shape each of these kernels is a few microseconds, so grid launch latency and CTA
 // start-up are a large share of the chain; PDL overlaps them with the predecessor's execution.  MOCO_PDL=0 turns
@@ -62,7 +73,7 @@ inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
     attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
-    return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
+    return counted(cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...));
 }
 
 inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }

@@ -290,7 +290,7 @@ static cudaError_t launch_bn(const void* x, const void* w, void* y, int M, int C
         }
     }
     conv1x1_stats_kernel<BN><<<dim3(slices, a.R), kCvThreads, smem, stream>>>(tm_x, tm_w, tm_y, a);
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t launch_conv1x1_bn_stats(const void* x, const void* w, void* y, long long M, int Cin, int Cout,
@@ -506,7 +506,7 @@ static cudaError_t launch_apply(const void* x, const void* w, const void* res, v
         }
     }
     conv1x1_bn_apply_kernel<BN, SC><<<dim3(slices, R), kCvThreads, smem, stream>>>(tm_x, tm_w, tm_r, tm_y, a);
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t launch_conv1x1_bn_add_relu(const void* x, const void* w, const void* res, void* y, void* mask, long long M,
@@ -801,7 +801,7 @@ cudaError_t launch_conv1x1_dgrad_bn_bwd(const void* dh, const void* w, void* g, 
     }
     conv1x1_dgrad_bn_bwd_kernel<<<dim3(slices, a.R), kCvThreads, smem, stream>>>(tm_dh, tm_w, tm_x, tm_dy2, tm_mask,
                                                                                   tm_g, a);
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace moco

@@ -98,7 +98,7 @@ cudaError_t launch_ema(const void* segs, const int* chunk_prefix, int n_segs, in
     int blocks = n_chunks < 132 * 8 ? n_chunks : 132 * 8;
     ema_multi_kernel<<<blocks, kEmaThreads, 0, stream>>>(static_cast<const EmaSeg*>(segs), chunk_prefix, n_segs, n_chunks,
                                                          m, one_minus_m);
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace moco

@@ -144,7 +144,7 @@ cudaError_t launch_combine_partial(int N, int C, int slices, int n_pad, float2* 
     if (exact.row_exact != nullptr && C > kSimtMaxC) return cudaErrorNotSupported;
     combine_partial_kernel<<<(N + kPartialRows - 1) / kPartialRows, kPartialRows * 32, 0, stream>>>(
         N, C, slices, n_pad, ws.part_ms, ms_out, exact);
-    return cudaGetLastError();
+    return launched();
 }
 
 // sharded queue, step 2: merge the W ranks' (max, sum) [W, N] with the positive logit (ws.lpos) -> lse, loss, prob
@@ -153,7 +153,7 @@ cudaError_t launch_combine_merge(int N, int world, float inv_T, const float2* ms
     const int rows_per_block = 8;
     combine_kernel<<<(N + rows_per_block - 1) / rows_per_block, rows_per_block * 32, 0, stream>>>(
         N, 0, 0, world, N, inv_T, ws.lpos, ms_all, nullptr, lse, loss_rows, prob_rows, loss_prob, ws.counters);
-    return cudaGetLastError();
+    return launched();
 }
 
 // o_partial_i = sum_{j in shard} p_ij shard_j of one row, exactly (out of line: the common path keeps its registers)
@@ -279,7 +279,7 @@ cudaError_t launch_dq_finish_peers(const void* const* peers_host, int world, int
     if (threads > 256) threads = 256;
     if (threads < 32) threads = 32;
     dq_finish_peers_kernel<<<N, threads, 0, stream>>>(t, world, rank * N, N, C, inv_T, k, k_dtype, prob_rows, dq);
-    return cudaGetLastError();
+    return launched();
 }
 
 // ---------------------------------------------------------------------------
@@ -326,7 +326,7 @@ cudaError_t launch_simt_rows(const __nv_bfloat16* q_bf16, const void* k, int k_d
     if (C > kSimtMaxC) return cudaErrorNotSupported;
     simt_rows_kernel<<<N, kSimtThreads, 0, stream>>>(q_bf16, k, k_dtype, queue, N, C, K, inv_T, ws.lpos, logits,
                                                      lse, loss_rows, prob_rows, loss_prob, dq, ws.counters);
-    return cudaGetLastError();
+    return launched();
 }
 
 // ---------------------------------------------------------------------------
@@ -380,7 +380,7 @@ cudaError_t launch_bwd_dense(const float* g, const void* k, int k_dtype, const _
     int threads = C >= 256 ? 256 : ((C + 31) / 32 * 32);
     dim3 grid((N + kDenseRows - 1) / kDenseRows, (C + threads - 1) / threads);
     bwd_dense_kernel<<<grid, threads, 0, stream>>>(g, k, k_dtype, queue, N, C, K, inv_T, dq);
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace moco

@@ -301,7 +301,7 @@ cudaError_t launch_maxpool_fwd(const void* x, void* y, void* idx, int N, int H, 
     if (bn) maxpool3x3s2_fwd_kernel<1><<<pool_grid(a), kPoolThreads, smem, stream>>>(a);
     else if (ev) maxpool3x3s2_fwd_kernel<2><<<pool_grid(a), kPoolThreads, smem, stream>>>(a);
     else maxpool3x3s2_fwd_kernel<0><<<pool_grid(a), kPoolThreads, 0, stream>>>(a);
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t launch_maxpool_bwd(const void* dy, const void* dy2, const void* idx, void* dx, int N, int H, int W, int C,
@@ -312,7 +312,7 @@ cudaError_t launch_maxpool_bwd(const void* dy, const void* dy2, const void* idx,
     a.idx = const_cast<uint2*>(static_cast<const uint2*>(idx));
     if (dy2 != nullptr) maxpool3x3s2_bwd_kernel<true><<<pool_grid(a), kPoolThreads, 0, stream>>>(a);
     else maxpool3x3s2_bwd_kernel<false><<<pool_grid(a), kPoolThreads, 0, stream>>>(a);
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace moco

@@ -133,7 +133,7 @@ cudaError_t launch_f32_to_bf16(const float* src, __nv_bfloat16* dst, size_t n, c
     if (blocks > 132 * 16) blocks = 132 * 16;
     if (blocks == 0) blocks = 1;
     f32_to_bf16_kernel<<<(int)blocks, 256, 0, stream>>>(src, dst, n);
-    return cudaGetLastError();
+    return launched();
 }
 
 // ---------------------------------------------------------------------------
@@ -360,7 +360,7 @@ cudaError_t launch_gather(const void* const* peers_host, int world, int rows_per
     if (n_rows == 0) {
         if (sa.epoch == 0u) return cudaSuccess;
         signal_barrier_kernel<<<1, 32, 0, stream>>>(sa);   // still a participant of the event
-        return cudaGetLastError();
+        return launched();
     }
     PeerTable t;
     for (int i = 0; i < kMaxWorld; ++i) t.base[i] = i < world ? static_cast<const char*>(peers_host[i]) : nullptr;
@@ -368,7 +368,11 @@ cudaError_t launch_gather(const void* const* peers_host, int world, int rows_per
     // load/store kernel above that (fp32 images, 602 KB rows)
     const bool use_ldg = (flags & 1) || row_bytes > (size_t)400 * 1024;
     if (row_bytes >= (size_t)kChunk / 2 && use_ldg) {
-        if (sa.epoch != 0u) signal_barrier_kernel<<<1, 32, 0, stream>>>(sa);
+        if (sa.epoch != 0u) {
+            signal_barrier_kernel<<<1, 32, 0, stream>>>(sa);
+            const cudaError_t e = launched();
+            if (e != cudaSuccess) return e;
+        }
         unsigned long long vec = row_bytes / 16;
         int gx = (int)((vec + 256 * 4 - 1) / (256 * 4));
         if (gx > 8) gx = 8;
@@ -399,13 +403,13 @@ cudaError_t launch_gather(const void* const* peers_host, int world, int rows_per
             gather_small_kernel<<<blocks, rows_per_block * 32, 0, stream>>>(t, rows_per_rank, src_rows, n_rows, vec,
                                                                            static_cast<uint4*>(dst));
     }
-    return cudaGetLastError();
+    return launched();
 }
 
 cudaError_t launch_signal_barrier(void* const* pads_host, int world, int rank, uint32_t epoch, cudaStream_t stream) {
     if (world > kMaxWorld) return cudaErrorInvalidValue;
     signal_barrier_kernel<<<1, 32, 0, stream>>>(make_sync(pads_host, world, rank, epoch));
-    return cudaGetLastError();
+    return launched();
 }
 
 }  // namespace moco

@@ -125,7 +125,7 @@ static cudaError_t launch_cluster(Kern kern, int grid, int threads, int smem, in
     }
     cfg.attrs = attr;
     cfg.numAttrs = n;
-    return cudaLaunchKernelEx(&cfg, kern, tmap, args);
+    return counted(cudaLaunchKernelEx(&cfg, kern, tmap, args));
 }
 
 // plan + launch one templated kernel instance: `fill(slices)` finalises the argument struct

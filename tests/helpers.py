@@ -1,9 +1,48 @@
-"""Test helpers: oracle evaluation in K-chunks (memory-light at full BASELINE sizes), golden-vector loading."""
+"""Test helpers: oracle evaluation in K-chunks (memory-light at full BASELINE sizes), golden-vector loading, and the
+kernels torch.profiler sees a call launch."""
 import os
 
 import numpy as np
 
 from oracle import moco_oracle as O
+
+
+def profiled(fns, reset=None):
+    """[(result of fn(), names of the kernels it ran, its moco_launch_count() delta) for fn in fns], from one
+    torch.profiler window in which each fn() is called in turn and must launch nothing but this library's kernels.
+    Memcpy and memset activities are not kernels and are left out.  A sentinel kernel precedes every call and follows
+    the last; a window in which the profiler lost any of them is not evidence of anything, so it is redone (after
+    reset() restores the inputs, for calls that are not idempotent)."""
+    import pytest
+    import torch
+    from torch.autograd import DeviceType
+    from torch.profiler import ProfilerActivity, profile
+    from moco_b200 import _lib
+    for attempt in range(3):
+        if attempt and reset is not None:
+            reset()
+        torch.cuda.synchronize()
+        calls = []
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for fn in fns:
+                torch.cuda._sleep(1000)
+                torch.cuda.synchronize()
+                before = _lib.launches
+                out = fn()
+                torch.cuda.synchronize()
+                calls.append((out, _lib.launches - before))
+            torch.cuda._sleep(1000)
+            torch.cuda.synchronize()
+        kernels = sorted((ev for ev in prof.events()
+                          if ev.device_type == DeviceType.CUDA and not ev.name.startswith(("Memcpy", "Memset"))),
+                         key=lambda ev: ev.time_range.start)
+        marks = [i for i, ev in enumerate(kernels) if "spin_kernel" in ev.name]
+        if len(marks) == len(fns) + 1:
+            break
+    else:
+        pytest.fail("torch.profiler lost sentinel kernels three times")
+    return [(out, [ev.name for ev in kernels[a + 1:b]], counted)
+            for (out, counted), a, b in zip(calls, marks, marks[1:])]
 
 
 def oracle_head_chunked(q, k, memory, T, chunk=16384, want_dq=True):

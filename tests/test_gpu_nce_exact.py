@@ -25,6 +25,7 @@ import pytest
 import torch
 
 from oracle import moco_oracle as O
+from tests import helpers
 
 pytestmark = pytest.mark.gpu
 
@@ -171,31 +172,9 @@ def _kernel_label(name):
 
 
 def profiled(fn, reset=None):
-    """(result of fn(), Counter of this library's kernels that ran, _lib.launches delta).  Two sentinel kernels
-    bracket the window; a window in which the profiler lost either of them is not evidence of anything, so it is
-    redone (after reset() restores fn's inputs, for a fn that is not idempotent)."""
-    from torch.profiler import ProfilerActivity, profile
-    lib = _lib()
-    for attempt in range(3):
-        if attempt and reset is not None:
-            reset()
-        torch.cuda.synchronize()
-        before = lib.launches
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            torch.cuda._sleep(1000)
-            torch.cuda.synchronize()
-            out = fn()
-            torch.cuda.synchronize()
-            torch.cuda._sleep(1000)
-            torch.cuda.synchronize()
-        counted = lib.launches - before
-        names = [ev.name for ev in prof.events()]
-        if sum("spin_kernel" in n for n in names) == 2:
-            break
-    else:
-        pytest.fail("torch.profiler lost the sentinel kernels three times")
-    ran = collections.Counter(l for l in map(_kernel_label, names) if l is not None)
-    return out, ran, counted
+    """(result of fn(), Counter of this library's kernels that ran, _lib.launches delta): tests.helpers.profiled."""
+    out, kernels, counted = helpers.profiled([fn], reset)[0]
+    return out, collections.Counter(l for l in map(_kernel_label, kernels) if l is not None), counted
 
 
 def expected_kernels(N, C, inv_T, flags, want_dq, want_logits, f32):

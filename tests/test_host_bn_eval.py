@@ -53,8 +53,3 @@ def test_bn_relu_maxpool_eval_validates_its_arguments():
     assert _stem(lib, C=96) == -2 and b"power of two" in lib.moco_last_error()
     assert _stem(lib, C=4096) == -2
     assert _stem(lib, N=0) == -2 and _stem(lib, H=0) == -2 and _stem(lib, W=0) == -2
-
-
-def test_eval_entry_points_are_counted_as_one_launch_each():
-    assert all(_lib._Counting._PER_CALL[n] == 1
-               for n in ("moco_bn_eval_act", "moco_bn_relu_maxpool_eval", "moco_bn_eval_act_avgpool"))

@@ -29,7 +29,7 @@ def test_library_exports_every_declared_symbol():
     names = _header_symbols()
     assert len(names) >= 15
     assert sorted(_lib.SIGNATURES) == names, "moco_b200/_lib.py and include/moco_b200.h disagree"
-    raw = ctypes.CDLL(_lib.lib_path())                       # dlopen + dlsym, independent of the Python proxy
+    raw = ctypes.CDLL(_lib.lib_path())                       # a second dlopen, independent of _lib's handle
     for n in names:
         assert ctypes.cast(getattr(raw, n), ctypes.c_void_p).value
         assert callable(getattr(lib, n))
@@ -391,19 +391,39 @@ def test_memory_moco_copies_a_misaligned_view_before_the_kernels_see_it():
     assert _aligned16(ok) is ok
 
 
-@pytest.mark.parametrize("N,C,flags,dq,logits,f32,expect", [
-    (256, 128, 0, True, False, True, (2, True)),          # one sweep + tail
-    (256, 256, 0, True, False, True, (3, True)),          # + the bf16 copy of q
-    (256, 128, 512, True, False, False, (5, False)),      # prep, stats, combine, dq, dq_reduce
-    (256, 128, 0, False, False, False, (3, False)),       # no gradient: the statistics pass only
-    (256, 128, 0, True, True, False, (5, False)),         # dense logits
-    (256, 100, 0, True, False, False, (2, False)),        # C % 64 != 0: prep + CUDA-core rows
-    (256, 128, 1, True, False, False, (2, False)),        # FORCE_SIMT
-    (16896, 128, 0, True, False, False, (2, True)),       # 132 blocks of 128 rows: still the one sweep
-    (16897, 128, 0, True, False, False, (2, False)),      # more q blocks than SMs: the CUDA-core kernel
-    (16897, 256, 0, True, False, True, (2, False)),       # (its prep doubles as the bf16 copy)
-    (16897, 128, 512, True, False, False, (2, False)),
-])
-def test_head_launch_count_follows_the_dispatch(N, C, flags, dq, logits, f32, expect):
-    from moco_b200 import _lib
-    assert _lib._Counting._head_plan(N, C, 1 / 0.07, flags, dq, logits, f32, 132) == expect
+def _launch_statement_end(src, i):
+    """Index just past the `;` of the `<<<...>>>(...);` statement whose `<<<` is at i."""
+    i = src.index(">>>", i) + 3
+    depth = 0
+    while True:
+        depth += {"(": 1, ")": -1}.get(src[i], 0)
+        i += 1
+        if depth == 0 and src[i - 1] == ")":
+            return src.index(";", i) + 1
+
+
+def test_every_kernel_launch_is_counted():
+    """moco_launch_count() is right only if every kernel launch in csrc/ is counted where it happens: each
+    `<<<...>>>(...);` is followed by launched() before the next launch or return (a launch in the if-branch of an
+    if / else is covered by the check after the else-branch), and the only launch API called, cudaLaunchKernelEx,
+    is called inside counted() (launch_pdl, launch_cluster)."""
+    csrc = os.path.join(ROOT, "moco_b200", "csrc")
+    chevrons = launch_api = 0
+    for name in sorted(os.listdir(csrc)):
+        if not name.endswith((".cu", ".cuh")):
+            continue
+        src = re.sub(r"//[^\n]*|/\*.*?\*/", lambda m: "\n" * m.group().count("\n"),
+                     open(os.path.join(csrc, name)).read(), flags=re.S)
+        for m in re.finditer(r"<<<", src):
+            chevrons += 1
+            rest = src[_launch_statement_end(src, m.start()):]
+            if re.match(r"\s*}?\s*else\b", rest):
+                continue
+            after = re.search(r"launched\(\)|<<<|\breturn\b(?!\s+launched\(\))", rest)
+            where = f"{name}:{src.count(chr(10), 0, m.start()) + 1}"
+            assert after and after.group() == "launched()", f"{where}: launch not followed by launched()"
+        for m in re.finditer(r"\bcu(?:da)?Launch\w*\s*\(", src):
+            launch_api += 1
+            assert m.group().startswith("cudaLaunchKernelEx") and re.search(r"counted\(\s*$", src[:m.start()]), \
+                f"{name}:{src.count(chr(10), 0, m.start()) + 1}: {m.group()} outside counted()"
+    assert chevrons >= 30 and launch_api >= 2
