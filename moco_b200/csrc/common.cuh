@@ -171,6 +171,10 @@ void bn_bwd_reduce_plan(long long M, int C, long long* passes, long long* ppc, i
 // the statistics pass alone (bn_stats_kernel): bn's save_mean / save_invstd and running statistics
 cudaError_t launch_bn_stats(const void* x, long long M, int C, const BnLayer& bn, void* ws, cudaStream_t stream);
 size_t conv1x1_workspace_bytes();
+// the shapes each 1x1-convolution launcher takes (it returns cudaErrorNotSupported outside them)
+bool conv1x1_stats_shape_ok(long long M, int Cin, int Cout);
+bool conv1x1_apply_shape_ok(long long M, int Cin, int Cout);
+bool conv1x1_dgrad_shape_ok(long long M, int Cin, int Cout);
 cudaError_t launch_conv1x1_bn_stats(const void* x, const void* w, void* y, long long M, int Cin, int Cout,
                                     const BnLayer& bn, void* ws, cudaStream_t stream);
 // y = relu(bn(x . w^T) + r) recomputing the convolution (moco_conv1x1_bn_add_relu_fwd); given as in BnFwdPlan
@@ -210,6 +214,8 @@ struct NceTcParams {
     int slices;
     int n_pad;
 };
+// the C the wgmma kernels take (a multiple of 64 up to 256)
+bool nce_tc_shape_ok(int C);
 cudaError_t launch_nce_tc(NceTcParams& p, const NceWorkspace& ws, cudaStream_t stream);
 // the q.Queue^T sweep with the gradient partials (one-sweep mode when lse == nullptr) and the fused tail (nce_tail.cu)
 cudaError_t launch_nce_sweep(const void* q, int q_dtype, int normalize, const __nv_bfloat16* queue, int N, int C, int K,

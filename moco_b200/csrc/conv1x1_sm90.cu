@@ -293,11 +293,14 @@ static cudaError_t launch_bn(const void* x, const void* w, void* y, int M, int C
     return launched();
 }
 
+bool conv1x1_stats_shape_ok(long long M, int Cin, int Cout) {
+    return M >= 1 && M <= 0x7fffff80LL && Cin >= 64 && Cin % 64 == 0 && Cin <= 65536 && Cout >= 64 && Cout % 64 == 0 &&
+           Cout <= 4096;
+}
+
 cudaError_t launch_conv1x1_bn_stats(const void* x, const void* w, void* y, long long M, int Cin, int Cout,
                                     const BnLayer& bn, void* ws, cudaStream_t stream) {
-    if (M < 1 || M > 0x7fffff80LL || Cin < 64 || Cin % 64 != 0 || Cin > 65536 || Cout < 64 || Cout % 64 != 0 ||
-        Cout > 4096)
-        return cudaErrorNotSupported;
+    if (!conv1x1_stats_shape_ok(M, Cin, Cout)) return cudaErrorNotSupported;
     if (Cout % 128 == 0) return launch_bn<128>(x, w, y, (int)M, Cin, Cout, bn, ws, stream);
     return launch_bn<64>(x, w, y, (int)M, Cin, Cout, bn, ws, stream);
 }
@@ -509,13 +512,16 @@ static cudaError_t launch_apply(const void* x, const void* w, const void* res, v
     return launched();
 }
 
+// Cout is the BatchNorm's C (a power of two in [64, 2048]), as in the statistics and apply passes it replaces
+bool conv1x1_apply_shape_ok(long long M, int Cin, int Cout) {
+    return M >= 1 && M <= 0x7fffff80LL && Cin >= 64 && Cin % 64 == 0 && Cin <= 65536 && Cout >= 64 && Cout <= 2048 &&
+           (Cout & (Cout - 1)) == 0;
+}
+
 cudaError_t launch_conv1x1_bn_add_relu(const void* x, const void* w, const void* res, void* y, void* mask, long long M,
                                        int Cin, int Cout, const BnLayer& bn, const BnLayer* sc, int given, void* ws,
                                        cudaStream_t stream) {
-    // Cout is the BatchNorm's C (a power of two in [64, 2048]), as in the statistics and apply passes it replaces
-    if (M < 1 || M > 0x7fffff80LL || Cin < 64 || Cin % 64 != 0 || Cin > 65536 || Cout < 64 || Cout > 2048 ||
-        (Cout & (Cout - 1)) != 0)
-        return cudaErrorNotSupported;
+    if (!conv1x1_apply_shape_ok(M, Cin, Cout)) return cudaErrorNotSupported;
     const int BN = Cout % 128 == 0 ? 128 : 64;
     cudaError_t e = cudaSuccess;
     if (!(given & MOCO_BN_STATS_GIVEN))                    // the statistics pass without storing h
@@ -759,13 +765,16 @@ static bool make_tmap_u8(CUtensorMap* m, const void* base, int rows, int cols, i
     return true;
 }
 
+// Cin is the BatchNorm's C (a power of two in [128, 2048]); Cout the GEMM's K
+bool conv1x1_dgrad_shape_ok(long long M, int Cin, int Cout) {
+    return M >= 1 && M <= 0x7fffff80LL && Cin >= kDgBN && Cin <= 2048 && (Cin & (Cin - 1)) == 0 && Cout >= 64 &&
+           Cout % 64 == 0 && Cout <= 4096;
+}
+
 cudaError_t launch_conv1x1_dgrad_bn_bwd(const void* dh, const void* w, void* g, long long M, int Cin, int Cout,
                                         const void* x, const void* mask, const void* dy2, const BnLayer& bn, void* ws,
                                         cudaStream_t stream) {
-    // Cin is the BatchNorm's C (a power of two in [128, 2048]); Cout the GEMM's K
-    if (M < 1 || M > 0x7fffff80LL || Cin < kDgBN || Cin > 2048 || (Cin & (Cin - 1)) != 0 || Cout < 64 ||
-        Cout % 64 != 0 || Cout > 4096)
-        return cudaErrorNotSupported;
+    if (!conv1x1_dgrad_shape_ok(M, Cin, Cout)) return cudaErrorNotSupported;
     using S = DgradShape;
     DgradArgs a{};
     a.M = (int)M; a.K = Cout;

@@ -391,12 +391,14 @@ static SweepArgs sweep_args(const void* q, int q_dtype, int normalize, int N, in
     return a;
 }
 
+bool nce_tc_shape_ok(int C) { return C % 64 == 0 && C >= 64 && C <= 256; }
+
 // lse == nullptr selects the one-sweep mode (the kernel also writes ws.part_ms).
 // plan_only: launch nothing, just report the slice count / padded rows this shape gets.
 cudaError_t launch_nce_sweep(const void* q, int q_dtype, int normalize, const __nv_bfloat16* queue, int N, int C, int K,
                              float inv_T, const float* lse, int num_sms, int* slices_out, int* n_pad_out,
                              const NceWorkspace& ws, cudaStream_t stream, bool plan_only) {
-    if (C % 64 != 0 || C < 64 || C > 256 || N < 1 || K < 1) return cudaErrorNotSupported;
+    if (!nce_tc_shape_ok(C) || N < 1 || K < 1) return cudaErrorNotSupported;
     if (normalize && C > 128) return cudaErrorNotSupported;          // the in-kernel norm needs a row in one warp
     if ((reinterpret_cast<uintptr_t>(q) & 15) != 0) return cudaErrorNotSupported;
     const int mblks = (N + kRowsPerCta - 1) / kRowsPerCta;
@@ -410,7 +412,7 @@ cudaError_t launch_nce_sweep(const void* q, int q_dtype, int normalize, const __
 }
 
 cudaError_t launch_nce_tc(NceTcParams& p, const NceWorkspace& ws, cudaStream_t stream) {
-    if (p.C % 64 != 0 || p.C < 64 || p.C > 256 || p.N < 1 || p.K < 1) return cudaErrorNotSupported;
+    if (!nce_tc_shape_ok(p.C) || p.N < 1 || p.K < 1) return cudaErrorNotSupported;
     const int G = p.cta_group;
     const int mblks = (p.N + kRowsPerCta * G - 1) / (kRowsPerCta * G);
     if (mblks * G > p.num_sms) return cudaErrorNotSupported;
