@@ -1,8 +1,15 @@
 """Linear evaluation of a pretrained encoder -- the train / validate loop of bl0/moco's ``eval.py`` (eval.py:188-360)
 on this package: a frozen ResNet-50 (``MoCoResNet.freeze()``, whose BatchNorms run on the eval kernels) feeds the
 features of ``--layer`` to the reference's linear classifier (``moco_b200.linear_eval``), trained with SGD (lr 30,
-momentum 0.9, no weight decay) and cross-entropy; top-1 / top-5 accuracy.  Synthetic images and labels stand in for
-the dataset (the reference's dataset, augmentation and LR schedule are out of scope).
+momentum 0.9, no weight decay) and cross-entropy; top-1 / top-5 accuracy.
+
+With ``--data-dir`` (``train/`` and ``val/`` image folders under it, as eval.py:119-120) it runs eval.py's recipe on
+real images: ``n_label`` is the folder's class count; the workers only decode (``moco_b200.augment.ImageFolderEval``)
+and the GPU applies the train crops (``augment_crops``, ``--aug``, ``--crop``) and the validation Resize(256) ->
+CenterCrop(224) (``resize_center_crops``); the learning rate follows eval.py's warm-up + cosine / step schedule per
+iteration (``moco_b200.linear_eval.get_scheduler``); every epoch trains, then validates over the whole validation set
+split across ranks without padding, and rank 0 prints ``* Acc@1 ... Acc@5 ... (n = ...)``.  Without ``--data-dir``
+synthetic images and labels stand in for the dataset (``--steps`` / ``--val-steps``, constant learning rate).
 
 ``--pretrained`` takes a checkpoint written by ``examples/train_moco.py --save`` or by the reference's ``train.py``:
 its ``model`` entry in either key naming, with or without the ``module.`` prefix.  Launch as train_moco.py
@@ -10,6 +17,7 @@ its ``model`` entry in either key naming, with or without the ``module.`` prefix
 DistributedDataParallel as eval.py:211 does.
 
     python examples/eval_linear.py --pretrained ckpt.pth --steps 20
+    torchrun --nproc_per_node 8 examples/eval_linear.py --pretrained ckpt.pth --data-dir /data/imagenet
 """
 import argparse
 import os
@@ -33,6 +41,17 @@ def parse_args(argv=None):
     ap.add_argument("--steps", type=int, default=20, help="training steps")
     ap.add_argument("--val-steps", type=int, default=2)
     ap.add_argument("--print-freq", type=int, default=10)
+    # real data (eval.py's flags and defaults); without --data-dir the synthetic loop above runs
+    ap.add_argument("--data-dir", default="", help="root with train/ and val/ image folders (default: synthetic data)")
+    ap.add_argument("--aug", default="NULL", choices=["NULL", "CJ"], help="train augmentation (eval.py: --aug)")
+    ap.add_argument("--crop", type=float, default=0.08, help="RandomResizedCrop's minimum scale")
+    ap.add_argument("--num-workers", type=int, default=4)
+    ap.add_argument("--epochs", type=int, default=100)
+    ap.add_argument("--lr-scheduler", default="cosine", choices=["step", "cosine"])
+    ap.add_argument("--warmup-epoch", type=int, default=5)
+    ap.add_argument("--warmup-multiplier", type=int, default=100)
+    ap.add_argument("--lr-decay-epochs", type=int, default=[30, 60, 90], nargs="+")
+    ap.add_argument("--lr-decay-rate", type=float, default=0.1)
     return ap.parse_args(argv)
 
 
@@ -67,6 +86,12 @@ def main(argv=None):
         if rank == 0:
             print(f"loaded {args.pretrained} (epoch {ckpt.get('epoch', '?')})", flush=True)
     model.freeze()
+    if args.data_dir:
+        res = run_data(args, model, dev, rank, world)
+        if world > 1:
+            dist.barrier()
+            dist.destroy_process_group()
+        return res
     classifier = LinearClassifierResNet(args.layer, args.num_classes, "avg", args.model_width).to(dev)
     criterion = torch.nn.CrossEntropyLoss()
     optimizer = torch.optim.SGD(classifier.parameters(), lr=args.learning_rate, momentum=args.momentum,
@@ -112,6 +137,74 @@ def main(argv=None):
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
+
+
+def run_data(args, model, dev, rank, world):
+    """eval.py:188-360 on the image folders under args.data_dir."""
+    import torch
+    from torch.utils.data import DataLoader, DistributedSampler
+    from moco_b200 import augment as A
+    from moco_b200.linear_eval import LinearClassifierResNet, ShardSampler, finish_validation, get_scheduler, val_totals
+
+    train_ds = A.ImageFolderEval(os.path.join(args.data_dir, "train"), train=True, scale=(args.crop, 1.0),
+                                 aug=args.aug)
+    val_ds = A.ImageFolderEval(os.path.join(args.data_dir, "val"), train=False)
+    batch = args.total_batch_size // world
+    train_sampler = DistributedSampler(train_ds, num_replicas=world, rank=rank)
+    train_loader = DataLoader(train_ds, batch_size=batch, sampler=train_sampler, num_workers=args.num_workers,
+                              pin_memory=True, drop_last=True, collate_fn=train_ds.collate_fn)
+    val_loader = DataLoader(val_ds, batch_size=batch, sampler=ShardSampler(len(val_ds), rank, world),
+                            num_workers=args.num_workers, pin_memory=True, drop_last=False,
+                            collate_fn=val_ds.collate_fn)
+    if len(train_loader) == 0:
+        raise ValueError(f"{len(train_ds)} training images give no full batch of {batch} per rank")
+    n_label = len(train_ds.classes)
+    if rank == 0:
+        print(f"train: {len(train_ds)} images, val: {len(val_ds)} images, {n_label} classes", flush=True)
+
+    classifier = LinearClassifierResNet(args.layer, n_label, "avg", args.model_width).to(dev)
+    criterion = torch.nn.CrossEntropyLoss()
+    optimizer = torch.optim.SGD(classifier.parameters(), lr=args.learning_rate, momentum=args.momentum,
+                                weight_decay=args.weight_decay)
+    scheduler = get_scheduler(optimizer, len(train_loader), args.epochs, args.lr_scheduler, args.warmup_epoch,
+                              args.warmup_multiplier, args.lr_decay_epochs, args.lr_decay_rate)
+    if world > 1:
+        classifier = torch.nn.parallel.DistributedDataParallel(classifier, device_ids=[args.local_rank],
+                                                               broadcast_buffers=False)
+
+    def features(x):
+        with torch.no_grad(), torch.autocast("cuda", dtype=torch.bfloat16):
+            return model(x, args.layer).float()
+
+    for epoch in range(1, args.epochs + 1):
+        train_sampler.set_epoch(epoch)
+        classifier.train()
+        for it, b in enumerate(train_loader):                                             # eval.py:254-311
+            x = A.augment_crops(b, dtype=torch.bfloat16, device=dev)
+            y = b[2].to(dev, non_blocking=True)
+            output = classifier(features(x))
+            loss = criterion(output, y)
+            optimizer.zero_grad()
+            loss.backward()
+            optimizer.step()
+            scheduler.step()
+            if rank == 0 and it % args.print_freq == 0:
+                print(f"epoch {epoch} [{it}/{len(train_loader)}]  lr {optimizer.param_groups[0]['lr']:.4g}  "
+                      f"loss {loss.item():.4f}", flush=True)
+
+        classifier.eval()                                                                 # eval.py:314-360
+        totals = torch.zeros(4, dtype=torch.float64, device=dev)
+        with torch.no_grad():
+            for b in val_loader:
+                x = A.resize_center_crops(b, dtype=torch.bfloat16, device=dev)
+                y = b[2].to(dev, non_blocking=True)
+                output = classifier(features(x))
+                totals += val_totals(output, y, criterion(output, y))
+        res = finish_validation(totals, len(val_ds))
+        if rank == 0:
+            print(f" * Acc@1 {res['acc'][0]:.3f} Acc@5 {res['acc'][1]:.3f} (n = {res['n']})  loss {res['loss']:.4f}",
+                  flush=True)
+    return res
 
 
 if __name__ == "__main__":

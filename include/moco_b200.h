@@ -29,7 +29,7 @@ extern "C" {
 #endif
 
 #define MOCO_B200_ABI_VERSION 3 /* 3: + moco_bn_*, moco_maxpool3x3s2_*, moco_crop_s2d_bf16, moco_conv1x1_*,
-                                    moco_augment_crops, moco_launch_count (additive) */
+                                    moco_augment_crops, moco_launch_count, moco_resize_center_crops (additive) */
 
 enum {
     MOCO_OK = 0,
@@ -553,6 +553,38 @@ typedef struct moco_aug_crop {
 
 int moco_augment_crops(const void* pixels, size_t pixels_bytes, const moco_aug_crop* crops, int n_crops, int out_h,
                        int out_w, const float* norm_host, void* dst, int dst_dtype, float* crop_means, void* stream);
+
+/* ------------------------------------------------------------------------
+ * The validation transform of the linear evaluation (eval.py:111-116: Resize(256) -> CenterCrop(224) -> ToTensor ->
+ * Normalize) from decoded uint8 images, in the conventions of moco_augment_crops above.
+ *
+ * Output image i is torchvision's TENSOR implementation applied to x = src_uint8 / 255 in fp32, with record
+ * windows[i]:
+ *   1. resize(x, [resized_h, resized_w], antialias=True): ATen's upsample_bilinear2d_aa of the WHOLE source image;
+ *   2. rows [top, top + out_h) and columns [left, left + out_w) of the resized image (center_crop's window).  Only the
+ *      window is computed: the resized image is never materialised;
+ *   3. (x - mean[c]) / std[c] (norm_host = {mean[3], std[3]}, a HOST array).
+ * The host fills the record with torchvision's arithmetic (moco_b200.augment.resize_window_params): Resize(int) keeps
+ * the short side at `resize` and sets the long side to int(resize * long / short); CenterCrop's offset is
+ * int(round((resized - out) / 2.0)), Python's round half to even.  Same fp32 operation order and the same deviation
+ * from PIL as moco_augment_crops; results agree with torchvision to fp32 rounding.
+ *
+ * pixels: packed uint8 HWC RGB images, image i at byte windows[i].src_offset.  windows: DEVICE array of n records.
+ * dst: image i at dst + i * 3 * out_h * out_w elements, MOCO_F32 or MOCO_BF16 (round-to-nearest-even of the fp32
+ * value): an [n, 3, out_h, out_w] tensor.  out_h, out_w in [1, 1024]; n in [0, 65535]; a source at most
+ * 1000 * resized_w pixels wide.  The records are validated on the host by the caller; here the window is clamped into
+ * the resized image and every source index into its own image and into [0, pixels_bytes), so a malformed record gives
+ * unspecified values but never reads outside the buffer.  One launch; deterministic.
+ * ---------------------------------------------------------------------- */
+typedef struct moco_resize_window {
+    int64_t src_offset;                   /* byte offset of the source image in `pixels`                 */
+    int32_t src_h, src_w;                 /* source image size                                           */
+    int32_t resized_h, resized_w;         /* size of the resized image the window is taken from          */
+    int32_t top, left;                    /* window origin in the resized image                          */
+} moco_resize_window;                     /* 32 bytes                                                    */
+
+int moco_resize_center_crops(const void* pixels, size_t pixels_bytes, const moco_resize_window* windows, int n,
+                             int out_h, int out_w, const float* norm_host, void* dst, int dst_dtype, void* stream);
 
 /* ------------------------------------------------------------------------
  * ShuffleBN row gather over NVLink peer memory.  Replaces dist_collect +

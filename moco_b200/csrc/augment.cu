@@ -24,6 +24,11 @@
 // One output row of one crop: the vertical pass reads the crop's source rows (contiguous uint8 HWC bytes, coalesced)
 // into a shared fp32 row v[x][c]; the horizontal pass gives each thread one output pixel.  A crop wider than kAugSpan
 // source pixels is processed in column chunks whose source span fits v.
+//
+// The validation transform (moco_resize_center_crops, eval.py:111-116: Resize -> CenterCrop -> Normalize) runs on the
+// same row pass: its "crop" is the whole source image resampled to resized_h x resized_w, and only the output window
+// [top, top + out_h) x [left, left + out_w) of that resized image is evaluated -- the window's origin is added to the
+// tap index (AugCtx::oy0 / ox0), which is 0 for the pre-training crops.  One kernel, no pointwise ops.
 #include "common.cuh"
 
 namespace moco {
@@ -113,10 +118,23 @@ struct AugCtx {
     unsigned long long base;            // byte index of the crop's top-left pixel
     unsigned long long row_bytes;       // src_w * 3
     int hh, ww;                         // crop box size
+    int oy0, ox0;                       // tap index of output row / column 0 (the resize window's top, left)
     int flags, order, cw;               // cw: output columns per chunk
     float sy, supy, invy, sx, supx, invx;
     float f[4], fm[4];                  // brightness, contrast, saturation, hue; fm[k] = fp32(1.0 - f[k])
 };
+
+// The resample of the c.hh x c.ww box to dst_h x dst_w (ATen's scale = in / out), of which out_w columns are computed.
+__device__ void aug_scales(AugCtx& c, int dst_h, int dst_w, int out_w) {
+    c.sy = (float)c.hh / (float)dst_h;
+    c.sx = (float)c.ww / (float)dst_w;
+    c.supy = c.sy >= 1.f ? c.sy : 1.f;
+    c.supx = c.sx >= 1.f ? c.sx : 1.f;
+    c.invy = c.sy >= 1.f ? (float)(1.0 / (double)c.sy) : 1.f;
+    c.invx = c.sx >= 1.f ? (float)(1.0 / (double)c.sx) : 1.f;
+    c.cw = out_w;
+    if (c.ww > kAugSpan) c.cw = max(1, min(out_w, (int)((float)(kAugSpan - 4) / c.sx) - 1));
+}
 
 __device__ AugCtx aug_ctx(const uint8_t* pix, unsigned long long pixels_bytes, const moco_aug_crop& cr, int out_h,
                           int out_w) {
@@ -130,16 +148,10 @@ __device__ AugCtx aug_ctx(const uint8_t* pix, unsigned long long pixels_bytes, c
     const unsigned long long off = cr.src_offset < 0 ? 0ULL : (unsigned long long)cr.src_offset;
     c.row_bytes = (unsigned long long)W * 3ULL;
     c.base = off + (unsigned long long)top * c.row_bytes + (unsigned long long)left * 3ULL;
+    c.oy0 = c.ox0 = 0;
     c.flags = cr.flags;
     c.order = cr.order;
-    c.sy = (float)c.hh / (float)out_h;
-    c.sx = (float)c.ww / (float)out_w;
-    c.supy = c.sy >= 1.f ? c.sy : 1.f;
-    c.supx = c.sx >= 1.f ? c.sx : 1.f;
-    c.invy = c.sy >= 1.f ? (float)(1.0 / (double)c.sy) : 1.f;
-    c.invx = c.sx >= 1.f ? (float)(1.0 / (double)c.sx) : 1.f;
-    c.cw = out_w;
-    if (c.ww > kAugSpan) c.cw = max(1, min(out_w, (int)((float)(kAugSpan - 4) / c.sx) - 1));
+    aug_scales(c, out_h, out_w, out_w);
     const float fs[4] = {cr.brightness, cr.contrast, cr.saturation, cr.hue};
 #pragma unroll
     for (int k = 0; k < 4; ++k) { c.f[k] = fs[k]; c.fm[k] = (float)(1.0 - (double)fs[k]); }
@@ -181,7 +193,7 @@ struct AugOut {                         // the apply pass's destination (dst == 
 // value to gsum.  xt: the crop's column taps.  All threads of the CTA call it.
 __device__ void aug_row(const AugCtx& c, const AugTap* xt, float* v, int oy, int out_w, const AugOut& o,
                         long long crop, float& gsum) {
-    const AugTap ty = aug_tap(oy, c.sy, c.supy, c.invy, c.hh);
+    const AugTap ty = aug_tap(c.oy0 + oy, c.sy, c.supy, c.invy, c.hh);
     for (int a = 0; a < out_w; a += c.cw) {
         const int e = min(a + c.cw, out_w);
         const int x0 = xt[a].lo;
@@ -241,7 +253,7 @@ struct AugArgs {
 };
 
 __device__ void aug_columns(const AugCtx& c, AugTap* xt, int out_w) {
-    for (int i = threadIdx.x; i < out_w; i += blockDim.x) xt[i] = aug_tap(i, c.sx, c.supx, c.invx, c.ww);
+    for (int i = threadIdx.x; i < out_w; i += blockDim.x) xt[i] = aug_tap(c.ox0 + i, c.sx, c.supx, c.invx, c.ww);
     __syncthreads();
 }
 
@@ -307,6 +319,69 @@ cudaError_t launch_augment(const void* pixels, size_t pixels_bytes, const moco_a
     cudaError_t e = launched();
     if (e != cudaSuccess) return e;
     aug_apply_kernel<<<dim3((out_h + kAugRows - 1) / kAugRows, n_crops), kAugThreads, 0, stream>>>(p);
+    return launched();
+}
+
+// One resize window's record, clamped like aug_ctx: the box is the whole source image, the resized size is at least
+// the output's and the window lies inside the resized image, so every tap index stays inside the image.
+__device__ AugCtx window_ctx(const uint8_t* pix, unsigned long long pixels_bytes, const moco_resize_window& wr,
+                             int out_h, int out_w) {
+    AugCtx c;
+    c.pix = pix;
+    c.last = pixels_bytes - 1;
+    c.hh = max(wr.src_h, 1);
+    c.ww = max(wr.src_w, 1);
+    const unsigned long long off = wr.src_offset < 0 ? 0ULL : (unsigned long long)wr.src_offset;
+    c.row_bytes = (unsigned long long)c.ww * 3ULL;
+    c.base = off;
+    const int rh = max(wr.resized_h, out_h), rw = max(wr.resized_w, out_w);
+    c.oy0 = min(max(wr.top, 0), rh - out_h);
+    c.ox0 = min(max(wr.left, 0), rw - out_w);
+    c.flags = 0;
+    c.order = 0;
+    aug_scales(c, rh, rw, out_w);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) { c.f[k] = 0.f; c.fm[k] = 1.f; }
+    return c;
+}
+
+struct ResizeArgs {
+    const uint8_t* pix;
+    unsigned long long pixels_bytes;
+    const moco_resize_window* windows;
+    int out_h, out_w;
+    float norm[6];
+    void* dst;
+    int dtype;
+};
+
+// rows [blockIdx.x * kAugRows, +kAugRows) of window blockIdx.y
+__global__ void __launch_bounds__(kAugThreads) resize_window_kernel(const __grid_constant__ ResizeArgs p) {
+    __shared__ AugTap xt[kAugMaxOut];
+    __shared__ float v[kAugSpan * 3];
+    const AugCtx c = window_ctx(p.pix, p.pixels_bytes, p.windows[blockIdx.y], p.out_h, p.out_w);
+    aug_columns(c, xt, p.out_w);
+    const AugOut o = {p.dst, p.dtype, (long long)p.out_h * p.out_w, p.norm, nullptr};
+    float unused = 0.f;
+    const int y1 = min((int)(blockIdx.x + 1) * kAugRows, p.out_h);
+    for (int oy = blockIdx.x * kAugRows; oy < y1; ++oy) aug_row(c, xt, v, oy, p.out_w, o, blockIdx.y, unused);
+}
+
+cudaError_t launch_resize_windows(const void* pixels, size_t pixels_bytes, const moco_resize_window* windows, int n,
+                                  int out_h, int out_w, const float norm[6], void* dst, int dst_dtype,
+                                  cudaStream_t stream) {
+    if (!augment_shape_ok(n, out_h, out_w)) return cudaErrorNotSupported;
+    if (n == 0) return cudaSuccess;
+    ResizeArgs p;
+    p.pix = static_cast<const uint8_t*>(pixels);
+    p.pixels_bytes = pixels_bytes;
+    p.windows = windows;
+    p.out_h = out_h;
+    p.out_w = out_w;
+    for (int k = 0; k < 6; ++k) p.norm[k] = norm[k];
+    p.dst = dst;
+    p.dtype = dst_dtype;
+    resize_window_kernel<<<dim3((out_h + kAugRows - 1) / kAugRows, n), kAugThreads, 0, stream>>>(p);
     return launched();
 }
 

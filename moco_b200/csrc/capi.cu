@@ -546,6 +546,27 @@ int moco_augment_crops(const void* pixels, size_t pixels_bytes, const moco_aug_c
                        "augment kernels");
 }
 
+int moco_resize_center_crops(const void* pixels, size_t pixels_bytes, const moco_resize_window* windows, int n,
+                             int out_h, int out_w, const float* norm, void* dst, int dst_dtype, void* stream_) {
+    g_err[0] = 0;
+    static_assert(sizeof(moco_resize_window) == 32, "moco_resize_window is 8 32-bit words ([n, 8] int32 on the host)");
+    const char* fn = "moco_resize_center_crops";
+    if (!norm || (dst_dtype != MOCO_F32 && dst_dtype != MOCO_BF16) ||
+        (n > 0 && (!pixels || pixels_bytes == 0 || !windows || !dst || !aligned(windows, 8) ||
+                   !aligned(dst, dst_dtype == MOCO_F32 ? 4 : 2))))
+        return refuse(fn, MOCO_ERR_INVALID, "bad argument (null or misaligned pointer, empty pixel buffer, or "
+                      "dst_dtype=%d)", dst_dtype);
+    for (int k = 0; k < 6; ++k)
+        if (!isfinite(norm[k]) || (k >= 3 && norm[k] == 0.f))
+            return refuse(fn, MOCO_ERR_INVALID, "norm must be finite mean[3], std[3] with std != 0");
+    if (!augment_shape_ok(n, out_h, out_w))
+        return refuse(fn, MOCO_ERR_INVALID, "needs n in [0, 65535] and out_h, out_w in [1, 1024] (n=%d out_h=%d "
+                      "out_w=%d)", n, out_h, out_w);
+    return cuda_result(launch_resize_windows(pixels, pixels_bytes, windows, n, out_h, out_w, norm, dst, dst_dtype,
+                                             static_cast<cudaStream_t>(stream_)),
+                       "resize window kernel");
+}
+
 int moco_maxpool3x3s2_fwd(const void* x, void* y, void* taps, int N, int H, int W, int C, void* stream_) {
     g_err[0] = 0;
     if (!ptr16(x) || !ptr16(y) || !taps || !aligned(taps, 8))

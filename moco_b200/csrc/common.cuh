@@ -190,6 +190,9 @@ bool augment_shape_ok(int n_crops, int out_h, int out_w);
 cudaError_t launch_augment(const void* pixels, size_t pixels_bytes, const moco_aug_crop* crops, int n_crops, int out_h,
                            int out_w, const float norm[6], void* dst, int dst_dtype, float* crop_means,
                            cudaStream_t stream);
+cudaError_t launch_resize_windows(const void* pixels, size_t pixels_bytes, const moco_resize_window* windows, int n,
+                                  int out_h, int out_w, const float norm[6], void* dst, int dst_dtype,
+                                  cudaStream_t stream);
 int ema_chunk_elems();
 cudaError_t launch_ema(const void* segs, const int* chunk_prefix, int n_segs, int n_chunks, float m,
                        float one_minus_m, cudaStream_t stream);
