@@ -11,8 +11,10 @@ iteration (``moco_b200.linear_eval.get_scheduler``); every epoch trains, then va
 split across ranks without padding, and rank 0 prints ``* Acc@1 ... Acc@5 ... (n = ...)``.  Without ``--data-dir``
 synthetic images and labels stand in for the dataset (``--steps`` / ``--val-steps``, constant learning rate).
 
-``--pretrained`` takes a checkpoint written by ``examples/train_moco.py --save`` or by the reference's ``train.py``:
-its ``model`` entry in either key naming, with or without the ``module.`` prefix.  Launch as train_moco.py
+``--pretrained`` takes a checkpoint written by ``examples/train_moco.py`` (``--save`` or the recipe's
+``--output-dir``) or by the reference's ``train.py``: its ``model`` entry in either key naming, with or without the
+``module.`` prefix.  It is read by ``moco_b200.checkpoint.load`` (weights only, the reference's ``opt`` Namespace
+allowed).  Launch as train_moco.py
 (``--local_rank`` / ``--local-rank`` / ``$LOCAL_RANK``); with more than one process the classifier is wrapped in
 DistributedDataParallel as eval.py:211 does.
 
@@ -67,6 +69,7 @@ def main(argv=None):
     args = parse_args(argv)
     import torch
     import torch.distributed as dist
+    from moco_b200 import checkpoint
     from moco_b200.encoders import from_reference_state_dict, resnet50
     from moco_b200.linear_eval import LinearClassifierResNet
 
@@ -81,7 +84,7 @@ def main(argv=None):
 
     model = resnet50(width=args.model_width).to(dev).to(memory_format=torch.channels_last)
     if args.pretrained:                                                                  # eval.py:149-153
-        ckpt = torch.load(args.pretrained, map_location="cpu")
+        ckpt = checkpoint.load(args.pretrained)
         model.load_state_dict(from_reference_state_dict(ckpt["model"]))
         if rank == 0:
             print(f"loaded {args.pretrained} (epoch {ckpt.get('epoch', '?')})", flush=True)

@@ -267,6 +267,24 @@ def augment_two_crop(batch, out_size=224, mean=MEAN, std=STD, dtype=torch.bfloat
     return out.view(n // 2, 6, out_h, out_w)
 
 
+def prefetch_pixels(batches, device=None):
+    """Yield each (pixels, params, ...) batch of ``batches`` with its pixels copied to ``device`` (default: the
+    current CUDA device) on a dedicated copy stream, so that the copy of batch i + 1 -- issued when the caller asks
+    for it, after queueing its work on batch i -- runs while that work does, instead of waiting for it on the
+    compute stream.  The current stream waits for the copy before anything it queues after the yield, and the
+    caching allocator keeps the device pixels until that stream is done with them.  The records stay on the host;
+    ``augment_crops`` / ``augment_two_crop`` take the batch as it is."""
+    dev = _device(device, "prefetch_pixels")
+    copy = torch.cuda.Stream(dev)
+    for batch in batches:
+        main = torch.cuda.current_stream(dev)
+        with torch.cuda.stream(copy):
+            pixels = batch[0].to(dev, non_blocking=True)
+        main.wait_stream(copy)
+        pixels.record_stream(main)
+        yield (pixels,) + tuple(batch[1:])
+
+
 def resize_center_crops(batch, resize=256, out=224, mean=MEAN, std=STD, dtype=torch.bfloat16,
                         device=None) -> torch.Tensor:
     """(pixels, windows, ...) from ``ImageFolderEval(train=False).collate_fn`` -> the [n, 3, out, out] batch of

@@ -80,6 +80,18 @@ class WarmupSchedule(LRScheduler):
     def get_lr(self):
         return [self.lr_at(base, self.last_epoch) for base in self.base_lrs]
 
+    def state_dict(self):
+        """LRScheduler's state without ``after``, a closure that cannot be pickled; the constructor rebuilds it."""
+        return {k: v for k, v in super().state_dict().items() if k != "after"}
+
+    def load_state_dict(self, state_dict):
+        """Restore a ``state_dict()``, or just ``{"last_epoch": t}`` to jump to iteration t, and set the optimizer's
+        learning rates to those of that iteration."""
+        super().load_state_dict({k: v for k, v in state_dict.items() if k != "after"})
+        self._last_lr = [self.lr_at(base, self.last_epoch) for base in self.base_lrs]
+        for group, lr in zip(self.optimizer.param_groups, self._last_lr):
+            group["lr"] = lr
+
 
 def get_scheduler(optimizer, n_iter_per_epoch: int, epochs: int, kind: str = "cosine", warmup_epoch: int = 5,
                   warmup_multiplier: float = 100, decay_epochs=(30, 60, 90), decay_rate: float = 0.1) -> WarmupSchedule:
