@@ -528,8 +528,11 @@ int moco_crop_gather_nhwc_bf16(const void* src, int src_dtype, long long src_ima
  *      stands before the contrast op; hue via _rgb2hsv / _hsv2rgb with the shifted hue taken % 1.0;
  *   4. hflip when flags has MOCO_AUG_FLIP;
  *   5. (x - mean[c]) / std[c], a subtraction then a division (norm_host = {mean[3], std[3]}, a HOST array).
- * Every step is fp32 in torchvision's operation order; the resample's sums are ordered differently from ATen's CPU
- * kernel (vertical pass first), so results agree with torchvision to fp32 rounding, not bit for bit.  The
+ * Every step is fp32 in torchvision's operation order, with three deviations in the resample: the vertical pass runs
+ * first (ATen's CPU kernel runs the horizontal one first), it sums the raw uint8 values and divides by 255 after
+ * the pass, and each weight is scaled by the correctly rounded reciprocal of the weights' sum instead of divided by
+ * it.  So results agree with torchvision to fp32 rounding, not bit for bit; oracle/augment_oracle.py restates the
+ * exact order, which the kernels match bit for bit, the contrast mean's reduction order included.  The
  * reference itself runs PIL on uint8, which rounds after every step: this is the documented deviation from it.
  *
  * pixels: packed uint8 HWC RGB images, image of crop i at byte crops[i].src_offset (src_h * src_w * 3 bytes).
