@@ -11,6 +11,18 @@ iteration (``moco_b200.linear_eval.get_scheduler``); every epoch trains, then va
 split across ranks without padding, and rank 0 prints ``* Acc@1 ... Acc@5 ... (n = ...)``.  Without ``--data-dir``
 synthetic images and labels stand in for the dataset (``--steps`` / ``--val-steps``, constant learning rate).
 
+The rest of eval.py's program comes with ``--data-dir`` only (INTEGRATION.md §5):
+
+* ``--output-dir D``: rank 0 writes ``D/config.json`` once and, after every epoch, the classifier checkpoint
+  ``D/current.pth`` (eval.py's keys, ``moco_b200.checkpoint.classifier_state``), plus ``D/ckpt_epoch_{e}.pth`` every
+  ``--save-freq`` epochs.  Without it nothing is written (eval.py's default is ``./output``).
+* ``--resume C`` continues from a classifier checkpoint of either project at its epoch + 1, with its momentum, its
+  best top-1 and the schedule at that epoch.  Epoch e's crops depend only on ``--rng-seed``, e, the rank and the
+  loader settings, so the resumed run ends with the ``current.pth`` of the uninterrupted one, bit for bit.
+* ``-e`` validates once (``--pretrained`` with the ``--resume`` classifier) and trains and writes nothing.
+* ``--dataset``, ``--model`` and ``--amp-opt-level`` are accepted so that eval.py's command lines parse; they have no
+  effect.
+
 ``--pretrained`` takes a checkpoint written by ``examples/train_moco.py`` (``--save`` or the recipe's
 ``--output-dir``) or by the reference's ``train.py``: its ``model`` entry in either key naming, with or without the
 ``module.`` prefix.  It is read by ``moco_b200.checkpoint.load`` (weights only, the reference's ``opt`` Namespace
@@ -20,6 +32,8 @@ DistributedDataParallel as eval.py:211 does.
 
     python examples/eval_linear.py --pretrained ckpt.pth --steps 20
     torchrun --nproc_per_node 8 examples/eval_linear.py --pretrained ckpt.pth --data-dir /data/imagenet
+    torchrun --nproc_per_node 4 examples/eval_linear.py --dataset imagenet --data-dir /data/imagenet \\
+        --pretrained-model ./output/current.pth --output-dir ./output/eval
 """
 import argparse
 import os
@@ -54,7 +68,29 @@ def parse_args(argv=None):
     ap.add_argument("--warmup-multiplier", type=int, default=100)
     ap.add_argument("--lr-decay-epochs", type=int, default=[30, 60, 90], nargs="+")
     ap.add_argument("--lr-decay-rate", type=float, default=0.1)
-    return ap.parse_args(argv)
+    ap.add_argument("--rng-seed", type=int, default=0, help="seeds the classifier's initialisation and the crop draws")
+    # the rest of eval.py's program, with --data-dir only
+    ap.add_argument("--output-dir", default="", help="config.json and the classifier checkpoints (default: write "
+                                                     "nothing; eval.py: ./output)")
+    ap.add_argument("--save-freq", type=int, default=5, help="also keep ckpt_epoch_{e}.pth every this many epochs")
+    ap.add_argument("--resume", default="", help="classifier checkpoint written by this script or by eval.py")
+    ap.add_argument("--start-epoch", type=int, default=None, help="first epoch (default 1; --resume sets it)")
+    ap.add_argument("-e", "--eval", action="store_true", help="only validate --pretrained with the --resume classifier")
+    # accepted so that the reference's command lines parse; the probe always runs bf16 autocast on a ResNet-50
+    ap.add_argument("--dataset", default="imagenet", choices=["imagenet", "imagenet100"], help="no effect")
+    ap.add_argument("--model", default="resnet50", choices=["resnet50"], help="no effect")
+    ap.add_argument("--amp-opt-level", default="O0", choices=["O0", "O1", "O2"], help="no effect")
+    args = ap.parse_args(argv)
+    if not args.data_dir:
+        given = [f for f, on in (("--resume", args.resume), ("-e", args.eval), ("--output-dir", args.output_dir),
+                                 ("--start-epoch", args.start_epoch is not None)) if on]
+        if given:
+            ap.error(f"{', '.join(given)}: only with --data-dir (the synthetic loop saves and resumes nothing)")
+    if args.start_epoch is None:
+        args.start_epoch = 1
+    if args.start_epoch < 1:
+        ap.error("--start-epoch must be at least 1")
+    return args
 
 
 def accuracy(output, target, topk=(1, 5)):
@@ -80,7 +116,7 @@ def main(argv=None):
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
         dist.init_process_group("nccl", device_id=dev)
     rank = dist.get_rank() if world > 1 else 0
-    torch.manual_seed(0)
+    torch.manual_seed(args.rng_seed)                                                      # eval.py:81-82
 
     model = resnet50(width=args.model_width).to(dev).to(memory_format=torch.channels_last)
     if args.pretrained:                                                                  # eval.py:149-153
@@ -143,19 +179,27 @@ def main(argv=None):
 
 
 def run_data(args, model, dev, rank, world):
-    """eval.py:188-360 on the image folders under args.data_dir."""
+    """eval.py:188-360 on the image folders under args.data_dir.  Returns the last validation's ``n``, ``loss`` and
+    ``acc`` with its ``epoch`` and the ``best_acc1`` so far; None when --resume or --start-epoch leaves no epoch to
+    run."""
     import torch
     from torch.utils.data import DataLoader, DistributedSampler
     from moco_b200 import augment as A
+    from moco_b200 import checkpoint
     from moco_b200.linear_eval import LinearClassifierResNet, ShardSampler, finish_validation, get_scheduler, val_totals
 
+    if rank == 0:
+        print(f"--dataset {args.dataset}, --model {args.model} and --amp-opt-level {args.amp_opt_level} have no "
+              "effect: the classes are the folder's, the encoder is a ResNet-50 and the probe runs under bf16 autocast",
+              flush=True)
     train_ds = A.ImageFolderEval(os.path.join(args.data_dir, "train"), train=True, scale=(args.crop, 1.0),
                                  aug=args.aug)
     val_ds = A.ImageFolderEval(os.path.join(args.data_dir, "val"), train=False)
     batch = args.total_batch_size // world
     train_sampler = DistributedSampler(train_ds, num_replicas=world, rank=rank)
     train_loader = DataLoader(train_ds, batch_size=batch, sampler=train_sampler, num_workers=args.num_workers,
-                              pin_memory=True, drop_last=True, collate_fn=train_ds.collate_fn)
+                              pin_memory=True, drop_last=True, collate_fn=train_ds.collate_fn,
+                              generator=torch.Generator())
     val_loader = DataLoader(val_ds, batch_size=batch, sampler=ShardSampler(len(val_ds), rank, world),
                             num_workers=args.num_workers, pin_memory=True, drop_last=False,
                             collate_fn=val_ds.collate_fn)
@@ -171,6 +215,14 @@ def run_data(args, model, dev, rank, world):
                                 weight_decay=args.weight_decay)
     scheduler = get_scheduler(optimizer, len(train_loader), args.epochs, args.lr_scheduler, args.warmup_epoch,
                               args.warmup_multiplier, args.lr_decay_epochs, args.lr_decay_rate)
+    start_epoch, best_acc1 = args.start_epoch, 0.0
+    if args.resume:                                                                       # eval.py:217-219
+        start_epoch, best_acc1 = checkpoint.restore_classifier(checkpoint.load(args.resume), classifier, optimizer)
+    if start_epoch > 1:
+        scheduler.load_state_dict({"last_epoch": (start_epoch - 1) * len(train_loader)})
+    if rank == 0 and args.resume:
+        print(f"resumed {args.resume}: epoch {start_epoch}, lr {optimizer.param_groups[0]['lr']:.6g}, "
+              f"best Acc@1 {best_acc1:.3f}", flush=True)
     if world > 1:
         classifier = torch.nn.parallel.DistributedDataParallel(classifier, device_ids=[args.local_rank],
                                                                broadcast_buffers=False)
@@ -179,8 +231,31 @@ def run_data(args, model, dev, rank, world):
         with torch.no_grad(), torch.autocast("cuda", dtype=torch.bfloat16):
             return model(x, args.layer).float()
 
-    for epoch in range(1, args.epochs + 1):
-        train_sampler.set_epoch(epoch)
+    def validate():                                                                       # eval.py:314-360
+        classifier.eval()
+        totals = torch.zeros(4, dtype=torch.float64, device=dev)
+        with torch.no_grad():
+            for b in val_loader:
+                x = A.resize_center_crops(b, dtype=torch.bfloat16, device=dev)
+                y = b[2].to(dev, non_blocking=True)
+                output = classifier(features(x))
+                totals += val_totals(output, y, criterion(output, y))
+        res = finish_validation(totals, len(val_ds))
+        if rank == 0:
+            print(f" * Acc@1 {res['acc'][0]:.3f} Acc@5 {res['acc'][1]:.3f} (n = {res['n']})  loss {res['loss']:.4f}",
+                  flush=True)
+        return res
+
+    if args.eval:                                                                         # eval.py:221-224
+        return {**validate(), "epoch": start_epoch - 1, "best_acc1": best_acc1}
+    save = bool(args.output_dir) and rank == 0
+    if save:
+        os.makedirs(args.output_dir, exist_ok=True)
+        checkpoint.write_config(args, args.output_dir)                                  # eval.py:371-377
+
+    res = None
+    for epoch in range(start_epoch, args.epochs + 1):
+        A.seed_epoch(train_loader, args.rng_seed, epoch, rank)                           # eval.py:234-235
         classifier.train()
         for it, b in enumerate(train_loader):                                             # eval.py:254-311
             x = A.augment_crops(b, dtype=torch.bfloat16, device=dev)
@@ -195,18 +270,12 @@ def run_data(args, model, dev, rank, world):
                 print(f"epoch {epoch} [{it}/{len(train_loader)}]  lr {optimizer.param_groups[0]['lr']:.4g}  "
                       f"loss {loss.item():.4f}", flush=True)
 
-        classifier.eval()                                                                 # eval.py:314-360
-        totals = torch.zeros(4, dtype=torch.float64, device=dev)
-        with torch.no_grad():
-            for b in val_loader:
-                x = A.resize_center_crops(b, dtype=torch.bfloat16, device=dev)
-                y = b[2].to(dev, non_blocking=True)
-                output = classifier(features(x))
-                totals += val_totals(output, y, criterion(output, y))
-        res = finish_validation(totals, len(val_ds))
-        if rank == 0:
-            print(f" * Acc@1 {res['acc'][0]:.3f} Acc@5 {res['acc'][1]:.3f} (n = {res['n']})  loss {res['loss']:.4f}",
-                  flush=True)
+        res = validate()
+        best_acc1 = max(best_acc1, res["acc"][0])
+        res.update(epoch=epoch, best_acc1=best_acc1)
+        if save:                                                                          # eval.py:244-246
+            checkpoint.save(checkpoint.classifier_state(args, epoch, classifier, best_acc1, optimizer, scheduler),
+                            args.output_dir, args.save_freq)
     return res
 
 

@@ -110,16 +110,10 @@ def make_recipe_loader(args, world, rank):
 
 
 def seed_epoch(loader, rng_seed, epoch, rank):
-    """Make epoch ``epoch``'s crop draws a function of (rng_seed, epoch, rank) alone: set the sampler's epoch and
-    seed the generator the next iterator draws its workers' seeds from -- or, without workers, the main process's
-    CPU generator, on which the dataset then draws."""
-    import numpy as np
-    import torch
-    loader.sampler.set_epoch(epoch)                                                      # train.py:213
-    seed = int(np.random.SeedSequence([rng_seed % 2 ** 64, epoch, rank]).generate_state(1, np.uint64)[0] >> 1)
-    loader.generator.manual_seed(seed)
-    if loader.num_workers == 0:
-        torch.default_generator.manual_seed(seed)
+    """``moco_b200.augment.seed_epoch``, which both example drivers use; imported when called, as this module's
+    other package imports are."""
+    from moco_b200.augment import seed_epoch
+    seed_epoch(loader, rng_seed, epoch, rank)
 
 
 def main(argv=None):

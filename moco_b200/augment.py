@@ -267,6 +267,18 @@ def augment_two_crop(batch, out_size=224, mean=MEAN, std=STD, dtype=torch.bfloat
     return out.view(n // 2, 6, out_h, out_w)
 
 
+def seed_epoch(loader, rng_seed: int, epoch: int, rank: int) -> None:
+    """Make epoch ``epoch``'s crop draws a function of (rng_seed, epoch, rank) alone: set the sampler's epoch and
+    seed the generator the next iterator draws its workers' seeds from -- or, without workers, the main process's
+    CPU generator, on which the dataset then draws.  ``loader`` needs its own ``generator`` and a sampler with
+    ``set_epoch``; workers must not be persistent, so that every epoch starts them afresh from that generator."""
+    loader.sampler.set_epoch(epoch)                                                      # train.py:213, eval.py:235
+    seed = int(np.random.SeedSequence([rng_seed % 2 ** 64, epoch, rank]).generate_state(1, np.uint64)[0] >> 1)
+    loader.generator.manual_seed(seed)
+    if loader.num_workers == 0:
+        torch.default_generator.manual_seed(seed)
+
+
 def prefetch_pixels(batches, device=None):
     """Yield each (pixels, params, ...) batch of ``batches`` with its pixels copied to ``device`` (default: the
     current CUDA device) on a dedicated copy stream, so that the copy of batch i + 1 -- issued when the caller asks
