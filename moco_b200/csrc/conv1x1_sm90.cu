@@ -1,25 +1,51 @@
-// 1x1 convolution forward on Hopper tensor cores (sm_90a) with the batch statistics of the following BatchNorm taken
-// in the epilogue: the bottleneck blocks' conv1 -> bn1, conv3 -> bn3 and stride-1 shortcut -> BatchNorm
-// (moco/models/resnet.py:74-102,139-143).  In NHWC a 1x1 / stride 1 convolution is the GEMM
-//     y[M, Cout] = x[M, Cin] . w[Cout, Cin]^T           (M = N*H*W; x, w, y bf16, fp32 accumulation, y rounded once)
-// and the statistics are those of y AS ROUNDED to bf16, the tensor the BatchNorm reads.  They replace that BatchNorm's
-// statistics pass (bn_nhwc.cu: bn_stats_kernel), which would read y back from HBM once more.
+// The bottleneck blocks' 1x1 convolutions on Hopper tensor cores (sm_90a), with BatchNorm work in their epilogues.
+// In NHWC a 1x1 / stride 1 convolution is a GEMM over the M = N*H*W pixel rows (bf16 operands, fp32 accumulation, each
+// output rounded to bf16 once).  Its three kernels share one skeleton.
 //
-// Layout of the work.  384 threads: warps 0-3 and 4-7 are two consumer warpgroups, each owning 64 rows of the CTA's
-// 128-row tile; one thread of warp 8 is the TMA producer (setmaxnreg: 40 / 232 registers per thread).  A CTA owns one
-// BN-column slice of y (BN = 128, or 64 when Cout is not a multiple of 128) and a contiguous range of 128-row tiles.
-// Per tile and 64-wide K chunk the producer loads the x slab [128 x 64] and the w slab [BN x 64] into a ring of smem
-// stages; each warpgroup runs wgmma m64nBNk16 x 4 from smem (both K-major, 128-byte swizzle).  The epilogue rounds the
-// accumulator to bf16, writes it into a double-buffered smem tile in the swizzled layout and stores it with one TMA
-// bulk store per warpgroup and 64 columns.
+// 384 threads: warps 0-3 and 4-7 are two consumer warpgroups, each owning 64 rows of the CTA's 128-row tile; one
+// thread of warp 8 is the TMA producer (setmaxnreg: 40 / 232 registers per thread).  A CTA owns one BN-column slice of
+// the output and a contiguous range of 128-row tiles.  Per tile and 64-wide K chunk the producer loads the A slab
+// [128 x 64] and the B slab (BN columns x 64) into a ring of smem stages; each warpgroup runs wgmma m64nBNk16 x 4 from
+// smem (A K-major, B K-major or MN-major, 128-byte swizzle) in increasing K, so every kernel that runs the mainloop
+// computes the same accumulator for the same tile.  The epilogue rounds the accumulator to bf16, stages it in smem in
+// the swizzled layout and stores it with TMA bulk stores.  A kernel whose epilogue reads operands other than the
+// accumulator has the producer load them into two buffers, one tile ahead of the consumers.  The BatchNorm reductions
+// read the staged bf16 tile back in the thread layout and fp32 order of the BatchNorm kernel they replace (bn_nhwc.cu),
+// and its per-CTA partials and fixed-order fp64 finish in the last CTA of a slab (bn_reduce.cuh) run on the consumers'
+// named barriers: bit-identical results.
 //
-// Statistics, bit-identical to bn_stats_kernel's on the same y.  The row ranges of the CTAs are those of the
-// statistics pass (bn_stats_plan: a chunk is a multiple of 256 rows, so whole tiles), and the 256 consumer threads read
-// the staged bf16 tile back from smem in that kernel's thread layout -- thread (v, rl) takes channels 8v .. 8v+7 of each
-// 64-channel slab in rows rl, rl + 32, ... in increasing order -- and add (y - y[0, c]) and its square in the same fp32
-// order.  The per-CTA partials and the fixed-order fp64 finish in the last CTA of a slab are bn_stats_kernel's own
-// (bn_reduce.cuh), on named barriers of the consumer threads.  y[0, c], the shift, is computed by every CTA: the CTAs
-// after the first run tile 0 once more, without storing it.
+// conv1x1_stats_kernel: y[M, Cout] = x[M, Cin] . w[Cout, Cin]^T for conv1 -> bn1, conv3 -> bn3 and the stride-1
+// shortcut -> BatchNorm (moco/models/resnet.py:74-102,139-143), with the batch statistics of y AS ROUNDED to bf16, the
+// tensor the BatchNorm reads.  They replace that BatchNorm's statistics pass (bn_stats_kernel), which would read y back
+// from HBM once more.  BN = 128, or 64 when Cout is not a multiple of 128.  Each warpgroup stages its 64 rows in a
+// double-buffered tile of its own and stores them with one TMA store per 64 columns.  The row ranges of the CTAs are
+// those of the statistics pass (bn_stats_plan: a chunk is a multiple of 256 rows, so whole tiles); thread (v, rl) takes
+// channels 8v .. 8v+7 of each 64-channel slab in rows rl, rl + 32, ... in increasing order and adds (y - y[0, c]) and
+// its square.  y[0, c], the shift, is computed by every CTA: the CTAs after the first run tile 0 once more, without
+// storing it.
+//
+// conv1x1_bn_apply_kernel: the residual BatchNorm applied in a second pass of the GEMM.  Once the statistics of
+// h = x . w^T are known (the kernel above), the block output y = relu(bn(h) + r) is computed from x again rather than
+// from h read back: for conv3 of a bottleneck (K = Cin = Cout / 4) the GEMM costs less than the 8 bytes per element of
+// h written and read.  The mainloop has the same BN as the statistics pass, so the accumulator of a tile is the one it
+// rounded.  The epilogue is bn_apply_kernel's arithmetic (bn_nhwc.cu): h rounded to bf16, z = fmaf(h, ca, cb) + r with
+// ca = gamma * invstd, cb = fmaf(-mean, ca, beta), ReLU, one rounding; with a shortcut BN r = bf16(fmaf(s, ca2, cb2) +
+// 0) of the shortcut convolution's raw output s.  The mask bytes (nullable) are relu_bits of the staged output.  The
+// epilogue operand is the r (or s) tile; y is staged in place over it and stored from there.  The grid is one wave: a
+// column slice per blockIdx.x, contiguous tile ranges per blockIdx.y.
+//
+// conv1x1_dgrad_bn_bwd_kernel: the input gradient with the producing BatchNorm's backward reduction.  The convolution's
+// input is the output of a block's residual BatchNorm, y = relu(bn(x) + r), and it has a second consumer, the next
+// block's residual branch, whose gradient dy2 is handed over (bn.py: hand_over).  The dgrad GEMM
+//     dX[M, Cin] = dH[M, Cout] . w[Cout, Cin]                 (w as stored is the MN-major B operand)
+// rounds dX to bf16 (what cuDNN's dgrad stores), adds dy2 with sum_grads' single rounding and applies the forward's
+// ReLU mask bits: g, the masked gradient that bn_bwd_reduce_kernel / bn_bwd_apply_kernel would form from the same
+// inputs.  g is written once (it is also the residual gradient of an identity block), and the reduction sums
+// sum g and sum g (x - mean) are taken from the staged tile in bn_bwd_reduce_kernel's row plan (bn_bwd_reduce_plan:
+// chunks of 128 rows, so whole tiles), thread layout and fp32 order, finished by its own code: bit-identical dbeta /
+// dgamma.  Only moco_bn_bwd_apply_given is left to run.  The epilogue operands are x, dy2 and the mask bytes of the
+// tile's 128 columns (66 KB per tile against 16-64 KB of mainloop operands); g is staged in place over dy2 and stored
+// from there.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -53,25 +79,27 @@ struct Conv1x1Args {
 
 template <int BN>
 struct Conv1x1Shape {
-    static constexpr int kA = kCvBM * 128;                 // x slab [128 rows x 64 bf16]
-    static constexpr int kB = BN * 128;                    // w slab [BN rows x 64 bf16]
+    static constexpr int kA = kCvBM * 128;                 // A slab [128 rows x 64 bf16]
+    static constexpr int kB = BN * 128;                    // B slab [BN x 64 bf16], or BN / 64 boxes [64 x 64 bf16]
     static constexpr int kStage = kA + kB;
     static constexpr int kOut = 64 * BN * 2;               // one warpgroup's [64 x BN] bf16 output tile
     static constexpr int kP = 2 * kBnSlab;                 // floats of a slab partial: two sums per channel
-    // output buffers, shift, slab_reduce scratch, slab_finish totals
+    // the statistics kernel's output buffers, shift, slab_reduce scratch, slab_finish totals
     static constexpr int kFixed = 4 * kOut + BN * 4 + 8 * kP * 4 + 8 * kP * 8;
 };
 
-// the barrier of the two consumer warpgroups
+// The consumers' named barriers (id 0 is __syncthreads'): both warpgroups, and warpgroup wg alone.
+__device__ __forceinline__ void consumer_sync() { named_bar_sync(3, kBnThreads); }
+__device__ __forceinline__ void warpgroup_sync(int wg) { named_bar_sync(1 + wg, 128); }
 struct ConsumerSync {
-    __device__ __forceinline__ void operator()() const { named_bar_sync(3, kBnThreads); }
+    __device__ __forceinline__ void operator()() const { consumer_sync(); }
 };
 
-// The mainloop of the forward kernels, one 128-row tile of column slice nb.  Producer: the Cin / 64 chunks of the x
-// slab and the w slab into the ring.  Consumers: wgmma over them in increasing K, so every kernel that runs it computes
-// the same accumulator for the same tile.  (st, ph): the ring position, carried from tile to tile.
-template <int BN>
-__device__ __forceinline__ void conv1x1_load_tile(const CUtensorMap* tm_x, const CUtensorMap* tm_w, uint8_t* ring,
+// The mainloop, one 128-row tile of column slice nb.  Producer: the ksteps chunks of the A slab and the B slab into the
+// ring.  B is K-major, one [BN x 64] box of w [N, K] as stored, or MN-major, BN / 64 boxes [64 x 64] of w [K, N] as
+// stored.  Consumers: wgmma over them in increasing K.  (st, ph): the ring position, carried from tile to tile.
+template <int BN, bool kBMnMajor>
+__device__ __forceinline__ void conv1x1_load_tile(const CUtensorMap* tm_a, const CUtensorMap* tm_b, uint8_t* ring,
                                                   uint64_t* full, uint64_t* empty, int NS, int& st, uint32_t& ph,
                                                   int tile, int nb, int ksteps) {
     using S = Conv1x1Shape<BN>;
@@ -79,23 +107,36 @@ __device__ __forceinline__ void conv1x1_load_tile(const CUtensorMap* tm_x, const
         mbar_wait(&empty[st], ph ^ 1u);
         mbar_arrive_expect_tx(&full[st], (uint32_t)S::kStage);   // OOB rows count too (zero-filled)
         uint8_t* s = ring + (size_t)st * S::kStage;
-        tma_load_2d(tm_x, &full[st], s, kc * 64, tile * kCvBM);
-        tma_load_2d(tm_w, &full[st], s + S::kA, kc * 64, nb * BN);
+        tma_load_2d(tm_a, &full[st], s, kc * 64, tile * kCvBM);
+        if constexpr (kBMnMajor) {
+#pragma unroll
+            for (int h = 0; h < BN / 64; ++h)
+                tma_load_2d(tm_b, &full[st], s + S::kA + h * 64 * 128, nb * BN + h * 64, kc * 64);
+        } else {
+            tma_load_2d(tm_b, &full[st], s + S::kA, kc * 64, nb * BN);
+        }
         if (++st == NS) { st = 0; ph ^= 1u; }
     }
 }
 
-template <int BN>
-__device__ __forceinline__ void conv1x1_mma_tile(float (&acc)[BN / 2], uint64_t a_desc0, uint64_t b_desc0, uint64_t* full,
+template <int BN, bool kBMnMajor>
+__device__ __forceinline__ void conv1x1_mma_tile(float (&acc)[BN / 2], const uint8_t* ring, int wg, uint64_t* full,
                                                  uint64_t* empty, int NS, int& st, uint32_t& ph, int ksteps, int t) {
-    constexpr uint64_t kStageUnits = Conv1x1Shape<BN>::kStage >> 4;
+    using S = Conv1x1Shape<BN>;
+    constexpr uint64_t kStageUnits = S::kStage >> 4;
+    constexpr uint64_t kBStep = kBMnMajor ? 128 : 2;              // k16 of B in 16-byte units: 16 rows, or 32 bytes
+    const uint64_t a_desc0 = make_sw128_desc(smem_u32(ring + wg * 64 * 128), 16, 1024);
+    const uint64_t b_desc0 = make_sw128_desc(smem_u32(ring + S::kA), kBMnMajor ? 64 * 128 : 16, 1024);
     int prev = 0;
     for (int kc = 0; kc < ksteps; ++kc) {
         mbar_wait(&full[st], ph);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k)
-            wgmma_ss<BN>(acc, a_desc0 + st * kStageUnits + 2 * k, b_desc0 + st * kStageUnits + 2 * k, (kc | k) != 0);
+        for (int k = 0; k < 4; ++k) {
+            const uint64_t a = a_desc0 + st * kStageUnits + 2 * k, b = b_desc0 + st * kStageUnits + kBStep * k;
+            if constexpr (kBMnMajor) wgmma_ss_tb<BN>(acc, a, b, (kc | k) != 0);
+            else                     wgmma_ss<BN>(acc, a, b, (kc | k) != 0);
+        }
         wgmma_commit();
         wgmma_wait<1>();                                          // the previous chunk's wgmmas have completed
         if (kc > 0 && t == 0) mbar_arrive(&empty[prev]);
@@ -105,6 +146,47 @@ __device__ __forceinline__ void conv1x1_mma_tile(float (&acc)[BN / 2], uint64_t 
     wgmma_wait<0>();
     reg_fence(acc);
     if (t == 0) mbar_arrive(&empty[prev]);
+}
+
+// The epilogue operands' two buffers of kBytes: the producer loads those of tile iteration it into buffer it & 1, one
+// tile ahead of the consumers, who hand the buffer back once the TMA store of the tile staged in it has read it.
+template <int kBytes>
+struct EpiRing {
+    uint8_t* buf;                                                  // [2][kBytes]
+    uint64_t* bar;                                                 // [2] full, [2] empty
+    __device__ __forceinline__ uint8_t* tile(int it) const { return buf + (it & 1) * kBytes; }
+    __device__ __forceinline__ uint64_t* full(int it) const { return &bar[it & 1]; }
+    __device__ __forceinline__ uint64_t* empty(int it) const { return &bar[2 + (it & 1)]; }
+    static __device__ __forceinline__ uint32_t parity(int it) { return (it >> 1) & 1; }
+    __device__ __forceinline__ void init() const {
+        for (int b = 0; b < 2; ++b) { mbar_init(full(b), 1); mbar_init(empty(b), kBnThreads); }
+    }
+    __device__ __forceinline__ void acquire(int it) const {      // producer, before its loads on full(it)
+        mbar_wait(empty(it), parity(it) ^ 1u);
+        mbar_arrive_expect_tx(full(it), (uint32_t)kBytes);        // OOB rows count too (zero-filled)
+    }
+    __device__ __forceinline__ void wait(int it) const { mbar_wait(full(it), parity(it)); }
+    __device__ __forceinline__ void release(int it) const {      // every consumer thread
+        if (threadIdx.x == 0) bulk_wait_read<0>();               // the store has read the tile out of the buffer
+        mbar_arrive(empty(it));
+    }
+};
+
+// The BatchNorm kernel's partials and finish, slab by slab, from sacc[s] (8 channels x 2 sums per consumer thread):
+// in the last CTA of slab s to arrive, threads j < kBnSlab call finish(j, s, c) for channel j of the slab, channel c
+// of the layer, with the slab totals in tot.
+template <int kSlabs, typename Finish>
+__device__ __forceinline__ void conv1x1_slabs_finish(float (&sacc)[kSlabs][16], float* red, double* tot, int* last,
+                                                     float* partial, unsigned int* counters, int nb, int r, int R,
+                                                     Finish finish) {
+#pragma unroll
+    for (int s = 0; s < kSlabs; ++s) {
+        const int gs = nb * kSlabs + s;
+        const float part = slab_reduce<2>(sacc[s], red, ConsumerSync());
+        if (slab_finish<2>(part, partial, counters + gs, gs, r, R, tot, last, ConsumerSync()) && threadIdx.x < kBnSlab)
+            finish((int)threadIdx.x, s, gs * kBnSlab + (int)threadIdx.x);
+        consumer_sync();                                          // red / tot are reused by the next slab
+    }
 }
 
 template <int BN>
@@ -148,7 +230,8 @@ conv1x1_stats_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_cons
             int st = 0;
             uint32_t ph = 0;
             for (int it = first; it < t1 - t0; ++it)
-                conv1x1_load_tile<BN>(&tm_x, &tm_w, ring, full, empty, NS, st, ph, it < 0 ? 0 : t0 + it, nb, ksteps);
+                conv1x1_load_tile<BN, false>(&tm_x, &tm_w, ring, full, empty, NS, st, ph, it < 0 ? 0 : t0 + it, nb,
+                                              ksteps);
         }
         return;
     }
@@ -158,8 +241,6 @@ conv1x1_stats_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_cons
     const int rloc = (warp & 3) * 16 + (lane >> 2);               // rows rloc and rloc + 8 of the warpgroup's 64
     const int ccol = 2 * (lane & 3);                              // first of this thread's two columns per 8
     const int v = threadIdx.x & (kBnLanes - 1), rl = threadIdx.x >> 3;   // bn_stats_kernel's thread layout
-    const uint64_t a_desc0 = make_sw128_desc(smem_u32(ring + wg * 64 * 128), 16, 1024);
-    const uint64_t b_desc0 = make_sw128_desc(smem_u32(ring + S::kA), 16, 1024);
     float acc[BN / 2];
     float sacc[kSlabs][16];                                       // per slab: 8 sums of (y - h), 8 of (y - h)^2
     float sh[kSlabs][8];
@@ -171,7 +252,7 @@ conv1x1_stats_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_cons
     uint32_t ph = 0;
     for (int it = first; it < t1 - t0; ++it) {
         const int tile = it < 0 ? 0 : t0 + it;
-        conv1x1_mma_tile<BN>(acc, a_desc0, b_desc0, full, empty, NS, st, ph, ksteps, t);
+        conv1x1_mma_tile<BN, false>(acc, ring, wg, full, empty, NS, st, ph, ksteps, t);
 
         if (it == first) {                                        // tile 0: the shift y[0, c], as rounded
             if (wg == 0 && warp == 0 && lane < 4) {
@@ -181,7 +262,7 @@ conv1x1_stats_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_cons
                     for (int e = 0; e < 2; ++e)
                         shift_s[8 * j + ccol + e] = __bfloat162float(__float2bfloat16_rn(acc[4 * j + e]));
             }
-            named_bar_sync(3, kBnThreads);
+            consumer_sync();
 #pragma unroll
             for (int s = 0; s < kSlabs; ++s)
 #pragma unroll
@@ -193,19 +274,19 @@ conv1x1_stats_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_cons
         uint8_t* buf = outb + (it & 1) * 2 * S::kOut;             // [warpgroup] halves of this tile
         uint8_t* ob = buf + wg * S::kOut;
         if (t == 0) bulk_wait_read<1>();                          // the store that last used this buffer has read it
-        named_bar_sync(1 + wg, 128);
+        warpgroup_sync(wg);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int row = rloc + 8 * h;
 #pragma unroll
             for (int j = 0; j < BN / 8; ++j) {
                 const __nv_bfloat162 q = __floats2bfloat162_rn(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
-                *reinterpret_cast<__nv_bfloat162*>(ob + (j >> 3) * 8192 + row * 128 + (((j & 7) ^ (row & 7)) << 4) +
-                                                   (lane & 3) * 4) = q;
+                uint8_t* p = ob + (j >> 3) * 8192 + sw128_offset(row, j & 7) + (lane & 3) * 4;
+                *reinterpret_cast<__nv_bfloat162*>(p) = q;
             }
         }
         fence_proxy_async();                                      // generic smem writes -> visible to the TMA store
-        named_bar_sync(3, kBnThreads);                            // both halves staged (and the buffer's last readers done)
+        consumer_sync();                                 // both halves staged (and the buffer's last readers done)
         if (t == 0 && a.store) {
 #pragma unroll
             for (int sl = 0; sl < BN / 64; ++sl)
@@ -216,8 +297,7 @@ conv1x1_stats_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_cons
         for (int p = 0; p < kCvBM / kBnRows; ++p) {
             const int row = p * kBnRows + rl;
             if (tile * kCvBM + row < a.M) {
-                const int lr = row & 63;
-                const uint8_t* src = buf + (row >> 6) * S::kOut + lr * 128 + ((v ^ (lr & 7)) << 4);
+                const uint8_t* src = buf + (row >> 6) * S::kOut + sw128_offset(row & 63, v);
 #pragma unroll
                 for (int s = 0; s < kSlabs; ++s) {
                     float f[8];
@@ -234,40 +314,58 @@ conv1x1_stats_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_cons
     }
     if (t == 0) bulk_wait<0>();
 
-    // ---- bn_stats_kernel's partials and finish, slab by slab
-#pragma unroll
-    for (int s = 0; s < kSlabs; ++s) {
-        const int gs = nb * kSlabs + s;
-        const float part = slab_reduce<2>(sacc[s], red, ConsumerSync());
-        if (slab_finish<2>(part, a.partial, a.counters + gs, gs, r, a.R, tot, last, ConsumerSync())) {
-            if (threadIdx.x < kBnSlab)
-                bn_stats_channel(tot, threadIdx.x, shift_s[s * kBnSlab + threadIdx.x], a.M, a.eps, a.momentum,
-                                 gs * kBnSlab + threadIdx.x, a.mean, a.invstd, a.running_mean, a.running_var);
-            if (gs == 0 && threadIdx.x == 0 && a.num_batches_tracked != nullptr) *a.num_batches_tracked += 1;
-        }
-        named_bar_sync(3, kBnThreads);                            // red / tot are reused by the next slab
-    }
+    conv1x1_slabs_finish(sacc, red, tot, last, a.partial, a.counters, nb, r, a.R, [&](int j, int s, int c) {
+        bn_stats_channel(tot, j, shift_s[s * kBnSlab + j], a.M, a.eps, a.momentum, c, a.mean, a.invstd, a.running_mean,
+                         a.running_var);
+        if (c == 0 && a.num_batches_tracked != nullptr) *a.num_batches_tracked += 1;
+    });
 }
 
 size_t conv1x1_workspace_bytes() { return 256 + (size_t)kCvMaxPartials * 2 * kBnSlab * sizeof(float); }
 
+// The ring's stage count and the kernel's dynamic smem: `fixed` bytes besides the ring, 256 bytes of mbarriers, and as
+// many stages of `stage` bytes as fit, at most 8.  With fewer than 2 the loads could not overlap the wgmmas.
+static cudaError_t ring_smem(int fixed, int stage, int* stages, int* smem) {
+    int n = (kSmemBudget - fixed - 256) / stage;
+    if (n > 8) n = 8;
+    if (n < 2) return cudaErrorNotSupported;
+    *stages = n;
+    *smem = n * stage + fixed + 256;
+    return cudaSuccess;
+}
+
+// The CTAs' row chunks of a BatchNorm pass's plan (bn_stats_plan, bn_bwd_reduce_plan), in 128-row tiles per CTA
+static int tiles_per_cta(void (*plan)(long long, int, long long*, long long*, int*), long long M, int C, int* R) {
+    long long passes = 0, ppc = 0;
+    plan(M, C, &passes, &ppc, R);
+    return (int)(ppc * kBnRows / kCvBM);
+}
+
+// Kern on a grid of kCvThreads-thread CTAs, its max-dynamic-smem attribute set first if this device needs it raised
+template <auto Kern, typename... Params>
+static cudaError_t launch_conv1x1(dim3 grid, int smem, cudaStream_t stream, const Params&... params) {
+    {
+        std::lock_guard<std::mutex> lock(g_kernel_cache_mutex);
+        const cudaError_t e = set_max_smem(Kern, kernel_cache<Kern>(), smem);
+        if (e != cudaSuccess) return e;
+    }
+    Kern<<<grid, kCvThreads, smem, stream>>>(params...);
+    return launched();
+}
+
 template <int BN>
-static cudaError_t launch_bn(const void* x, const void* w, void* y, int M, int Cin, int Cout, const BnLayer& bn,
-                             void* ws, cudaStream_t stream) {
+static cudaError_t launch_stats(const void* x, const void* w, void* y, int M, int Cin, int Cout, const BnLayer& bn,
+                                void* ws, cudaStream_t stream) {
     using S = Conv1x1Shape<BN>;
     Conv1x1Args a{};
     a.M = M; a.Cin = Cin;
     a.m_tiles = (M + kCvBM - 1) / kCvBM;
-    long long passes = 0, ppc = 0;
-    bn_stats_plan(M, Cout, &passes, &ppc, &a.R);           // the statistics pass's row chunks
-    a.ppc = (int)(ppc * kBnRows / kCvBM);
+    a.ppc = tiles_per_cta(bn_stats_plan, M, Cout, &a.R);   // the statistics pass's row chunks
     const int slices = Cout / BN, slabs = Cout / kBnSlab;
     if (slabs > kCvMaxSlabs || (long long)slabs * a.R > kCvMaxPartials) return cudaErrorNotSupported;
-    constexpr int kBarBytes = 256;
-    int stages = (kSmemBudget - S::kFixed - kBarBytes) / S::kStage;
-    if (stages > 8) stages = 8;
-    a.stages = stages;
-    const int smem = stages * S::kStage + S::kFixed + kBarBytes;
+    int smem = 0;
+    const cudaError_t e = ring_smem(S::kFixed, S::kStage, &a.stages, &smem);
+    if (e != cudaSuccess) return e;
     a.momentum = bn.momentum; a.eps = bn.eps;
     a.counters = static_cast<unsigned int*>(ws);
     a.partial = bn_ws_partials(ws);
@@ -279,18 +377,7 @@ static cudaError_t launch_bn(const void* x, const void* w, void* y, int M, int C
         return cudaErrorUnknown;
     if (y == nullptr) tm_y = tm_x;                         // not used
     else if (!make_tmap(&tm_y, y, M, Cout, 64)) return cudaErrorUnknown;
-    {
-        std::lock_guard<std::mutex> lock(g_kernel_cache_mutex);
-        KernelCache& kc = kernel_cache(BN / 64 - 1);
-        if (kc.smem_set < smem) {
-            cudaError_t e = cudaFuncSetAttribute(conv1x1_stats_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                 smem);
-            if (e != cudaSuccess) return e;
-            kc.smem_set = smem;
-        }
-    }
-    conv1x1_stats_kernel<BN><<<dim3(slices, a.R), kCvThreads, smem, stream>>>(tm_x, tm_w, tm_y, a);
-    return launched();
+    return launch_conv1x1<conv1x1_stats_kernel<BN>>(dim3(slices, a.R), smem, stream, tm_x, tm_w, tm_y, a);
 }
 
 bool conv1x1_stats_shape_ok(long long M, int Cin, int Cout) {
@@ -301,20 +388,11 @@ bool conv1x1_stats_shape_ok(long long M, int Cin, int Cout) {
 cudaError_t launch_conv1x1_bn_stats(const void* x, const void* w, void* y, long long M, int Cin, int Cout,
                                     const BnLayer& bn, void* ws, cudaStream_t stream) {
     if (!conv1x1_stats_shape_ok(M, Cin, Cout)) return cudaErrorNotSupported;
-    if (Cout % 128 == 0) return launch_bn<128>(x, w, y, (int)M, Cin, Cout, bn, ws, stream);
-    return launch_bn<64>(x, w, y, (int)M, Cin, Cout, bn, ws, stream);
+    if (Cout % 128 == 0) return launch_stats<128>(x, w, y, (int)M, Cin, Cout, bn, ws, stream);
+    return launch_stats<64>(x, w, y, (int)M, Cin, Cout, bn, ws, stream);
 }
 
 // ---- the residual BatchNorm applied in a second pass of the GEMM ----------------------------------------------------
-// Once the statistics of h = x . w^T are known (the pass above), the block output y = relu(bn(h) + r) is computed from
-// x again rather than from h read back: for conv3 of a bottleneck (K = Cin = Cout / 4) the GEMM costs less than the
-// 8 bytes per element of h written and read.  The mainloop is conv1x1_load_tile / conv1x1_mma_tile with the same BN,
-// so the accumulator of a tile is the one the statistics pass rounded and stored.  The epilogue is bn_apply_kernel's
-// arithmetic (bn_nhwc.cu): h rounded to bf16, z = fmaf(h, ca, cb) + r with ca = gamma * invstd, cb = fmaf(-mean, ca,
-// beta), ReLU, one rounding; with a shortcut BN r = bf16(fmaf(s, ca2, cb2) + 0) of the shortcut convolution's raw
-// output s.  The mask bytes (nullable) are relu_bits of the staged output.
-// The TMA producer loads the r (or s) tile into two buffers, one tile ahead of the consumers; y is staged in place over
-// it and stored from there.  The grid is one wave: a column slice per blockIdx.x, contiguous tile ranges per blockIdx.y.
 struct Conv1x1ApplyArgs {
     int M, Cin, C, m_tiles, ppc, stages;   // C = Cout; ppc = tiles per CTA
     const float* mean;
@@ -346,15 +424,14 @@ conv1x1_bn_apply_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_c
     if ((smem_u32(smem) & 1023u) != 0u) __trap();
     const int NS = a.stages;
     uint8_t* ring = smem;                                          // NS x (x slab, w slab)
-    uint8_t* epi = ring + (size_t)NS * S::kStage;                  // [2] r tiles, then y
+    uint8_t* epi = ring + (size_t)NS * S::kStage;
     float* ca = reinterpret_cast<float*>(epi + 2 * E::kTile);      // [BN] each
     float* cb = ca + BN;
     float* ca2 = cb + BN;
     float* cb2 = ca2 + BN;
     uint64_t* full = reinterpret_cast<uint64_t*>(cb2 + BN);
     uint64_t* empty = full + NS;
-    uint64_t* efull = empty + NS;
-    uint64_t* eempty = efull + 2;
+    const EpiRing<E::kTile> er{epi, empty + NS};                   // [2] r tiles, then y
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nb = blockIdx.x;
@@ -368,7 +445,7 @@ conv1x1_bn_apply_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_c
         tma_prefetch_desc(&tm_r);
         tma_prefetch_desc(&tm_y);
         for (int s = 0; s < NS; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
-        for (int b = 0; b < 2; ++b) { mbar_init(&efull[b], 1); mbar_init(&eempty[b], kBnThreads); }
+        er.init();
         fence_mbar_init();
     }
     if (threadIdx.x < BN) {                                        // bn_apply_kernel's coefficients
@@ -391,13 +468,12 @@ conv1x1_bn_apply_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_c
             int st = 0;
             uint32_t ph = 0;
             for (int it = 0; it < t1 - t0; ++it) {
-                const int tile = t0 + it, eb = it & 1;
-                mbar_wait(&eempty[eb], ((it >> 1) & 1) ^ 1u);
-                mbar_arrive_expect_tx(&efull[eb], (uint32_t)E::kTile);   // OOB rows count too (zero-filled)
+                const int tile = t0 + it;
+                er.acquire(it);
 #pragma unroll
                 for (int s = 0; s < kSlabs; ++s)
-                    tma_load_2d(&tm_r, &efull[eb], epi + eb * E::kTile + s * kSlab, nb * BN + s * 64, tile * kCvBM);
-                conv1x1_load_tile<BN>(&tm_x, &tm_w, ring, full, empty, NS, st, ph, tile, nb, ksteps);
+                    tma_load_2d(&tm_r, er.full(it), er.tile(it) + s * kSlab, nb * BN + s * 64, tile * kCvBM);
+                conv1x1_load_tile<BN, false>(&tm_x, &tm_w, ring, full, empty, NS, st, ph, tile, nb, ksteps);
             }
         }
         return;
@@ -408,26 +484,24 @@ conv1x1_bn_apply_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_c
     const int rloc = wg * 64 + (warp & 3) * 16 + (lane >> 2);    // tile rows rloc and rloc + 8
     const int ccol = 2 * (lane & 3);                              // first of this thread's two columns per 8
     const int v = threadIdx.x & (kBnLanes - 1), rl = threadIdx.x >> 3;   // 8-channel vector, row of the mask pass
-    const uint64_t a_desc0 = make_sw128_desc(smem_u32(ring + wg * 64 * 128), 16, 1024);
-    const uint64_t b_desc0 = make_sw128_desc(smem_u32(ring + S::kA), 16, 1024);
     const int mask_row = a.C >> 3;
     float acc[BN / 2];
     int st = 0;
     uint32_t ph = 0;
     for (int it = 0; it < t1 - t0; ++it) {
-        const int tile = t0 + it, eb = it & 1;
-        conv1x1_mma_tile<BN>(acc, a_desc0, b_desc0, full, empty, NS, st, ph, ksteps, t);
+        const int tile = t0 + it;
+        conv1x1_mma_tile<BN, false>(acc, ring, wg, full, empty, NS, st, ph, ksteps, t);
 
         // ---- epilogue: y = relu(fmaf(bf16(acc), ca, cb) + r), in place over r -> TMA store; mask bytes from the tile
-        uint8_t* e = epi + eb * E::kTile;
-        mbar_wait(&efull[eb], (it >> 1) & 1);
+        uint8_t* e = er.tile(it);
+        er.wait(it);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int row = rloc + 8 * h;
 #pragma unroll
             for (int j = 0; j < BN / 8; ++j) {
-                __nv_bfloat162* p = reinterpret_cast<__nv_bfloat162*>(e + (j >> 3) * kSlab + row * 128 +
-                                                                      (((j & 7) ^ (row & 7)) << 4) + (lane & 3) * 4);
+                __nv_bfloat162* p = reinterpret_cast<__nv_bfloat162*>(e + (j >> 3) * kSlab + sw128_offset(row, j & 7) +
+                                                                      (lane & 3) * 4);
                 const float2 r2 = __bfloat1622float2(*p);
                 float z[2];
 #pragma unroll
@@ -443,7 +517,7 @@ conv1x1_bn_apply_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_c
             }
         }
         fence_proxy_async();                                      // generic smem writes -> visible to the TMA store
-        named_bar_sync(3, kBnThreads);                            // the whole tile staged
+        consumer_sync();                                          // the whole tile staged
         if (threadIdx.x == 0) {
 #pragma unroll
             for (int s = 0; s < kSlabs; ++s) tma_store_2d(&tm_y, e + s * kSlab, nb * BN + s * 64, tile * kCvBM);
@@ -457,14 +531,13 @@ conv1x1_bn_apply_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_c
                 if (grow < a.M) {
 #pragma unroll
                     for (int s = 0; s < kSlabs; ++s) {
-                        const uint4 u = *reinterpret_cast<const uint4*>(e + s * kSlab + row * 128 + ((v ^ (row & 7)) << 4));
+                        const uint4 u = *reinterpret_cast<const uint4*>(e + s * kSlab + sw128_offset(row, v));
                         a.mask[grow * mask_row + nb * (BN / 8) + s * 8 + v] = (uint8_t)relu_bits(u);
                     }
                 }
             }
         }
-        if (threadIdx.x == 0) bulk_wait_read<0>();               // the store has read y out of the buffer
-        mbar_arrive(&eempty[eb]);
+        er.release(it);
     }
     if (threadIdx.x == 0) bulk_wait<0>();
 }
@@ -486,12 +559,9 @@ static cudaError_t launch_apply(const void* x, const void* w, const void* res, v
     if (R < 1) R = 1;
     a.ppc = (a.m_tiles + R - 1) / R;
     R = (a.m_tiles + a.ppc - 1) / a.ppc;
-    constexpr int kBarBytes = 256;
-    int stages = (kSmemBudget - E::kFixed - kBarBytes) / S::kStage;
-    if (stages > 8) stages = 8;
-    if (stages < 2) return cudaErrorNotSupported;
-    a.stages = stages;
-    const int smem = stages * S::kStage + E::kFixed + kBarBytes;
+    int smem = 0;
+    e = ring_smem(E::kFixed, S::kStage, &a.stages, &smem);
+    if (e != cudaSuccess) return e;
     a.mean = bn.save_mean; a.invstd = bn.save_invstd; a.gamma = bn.gamma; a.beta = bn.beta;
     if (SC) { a.mean2 = sc->save_mean; a.invstd2 = sc->save_invstd; a.gamma2 = sc->gamma; a.beta2 = sc->beta; }
     a.mask = static_cast<uint8_t*>(mask);
@@ -499,17 +569,7 @@ static cudaError_t launch_apply(const void* x, const void* w, const void* res, v
     if (!make_tmap(&tm_x, x, M, Cin, kCvBM) || !make_tmap(&tm_w, w, Cout, Cin, BN) ||
         !make_tmap(&tm_r, res, M, Cout, kCvBM) || !make_tmap(&tm_y, y, M, Cout, kCvBM))
         return cudaErrorUnknown;
-    {
-        std::lock_guard<std::mutex> lock(g_kernel_cache_mutex);
-        KernelCache& kc = kernel_cache(3 + 2 * (BN / 64 - 1) + (SC ? 1 : 0));
-        if (kc.smem_set < smem) {
-            e = cudaFuncSetAttribute(conv1x1_bn_apply_kernel<BN, SC>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-            if (e != cudaSuccess) return e;
-            kc.smem_set = smem;
-        }
-    }
-    conv1x1_bn_apply_kernel<BN, SC><<<dim3(slices, R), kCvThreads, smem, stream>>>(tm_x, tm_w, tm_r, tm_y, a);
-    return launched();
+    return launch_conv1x1<conv1x1_bn_apply_kernel<BN, SC>>(dim3(slices, R), smem, stream, tm_x, tm_w, tm_r, tm_y, a);
 }
 
 // Cout is the BatchNorm's C (a power of two in [64, 2048]), as in the statistics and apply passes it replaces
@@ -525,8 +585,8 @@ cudaError_t launch_conv1x1_bn_add_relu(const void* x, const void* w, const void*
     const int BN = Cout % 128 == 0 ? 128 : 64;
     cudaError_t e = cudaSuccess;
     if (!(given & MOCO_BN_STATS_GIVEN))                    // the statistics pass without storing h
-        e = BN == 128 ? launch_bn<128>(x, w, nullptr, (int)M, Cin, Cout, bn, ws, stream)
-                      : launch_bn<64>(x, w, nullptr, (int)M, Cin, Cout, bn, ws, stream);
+        e = BN == 128 ? launch_stats<128>(x, w, nullptr, (int)M, Cin, Cout, bn, ws, stream)
+                      : launch_stats<64>(x, w, nullptr, (int)M, Cin, Cout, bn, ws, stream);
     if (e == cudaSuccess && sc != nullptr && !(given & MOCO_BN_SC_STATS_GIVEN))
         e = launch_bn_stats(res, M, Cout, *sc, ws, stream);
     if (e != cudaSuccess) return e;
@@ -538,28 +598,13 @@ cudaError_t launch_conv1x1_bn_add_relu(const void* x, const void* w, const void*
 }
 
 // ---- backward: the input gradient with the producing BatchNorm's backward reduction ---------------------------------
-// The convolution's input is the output of a block's residual BatchNorm, y = relu(bn(x) + r), and it has a second
-// consumer, the next block's residual branch, whose gradient dy2 is handed over (bn.py: hand_over).  The dgrad GEMM
-//     dX[M, Cin] = dH[M, Cout] . w[Cout, Cin]                 (w as stored is the MN-major B operand: wgmma_ss_tb)
-// rounds dX to bf16 (what cuDNN's dgrad stores), adds dy2 with sum_grads' single rounding and applies the forward's
-// ReLU mask bits: g, the masked gradient that bn_bwd_reduce_kernel / bn_bwd_apply_kernel would form from the same
-// inputs.  g is written once (it is also the residual gradient of an identity block), and the reduction sums
-// sum g and sum g (x - mean) are taken from the staged tile in bn_bwd_reduce_kernel's row plan (bn_bwd_reduce_plan:
-// chunks of 128 rows, so whole tiles), thread layout and fp32 order, finished by its own code: bit-identical dbeta /
-// dgamma.  Only moco_bn_bwd_apply_given is left to run.
-// The epilogue operands (x, dy2 and the mask bytes of the tile's 128 columns: 66 KB per tile against 16-64 KB of
-// mainloop operands) are loaded by the TMA producer into two buffers, one tile ahead of the consumers.  g is staged in
-// place over dy2 and stored from there.
 constexpr int kDgBN = 128;                       // columns of dX per CTA
-struct DgradShape {
-    static constexpr int kA = kCvBM * 128;               // dH slab [128 rows x 64 bf16], K-major
-    static constexpr int kB = kDgBN * 128;               // w slab [64 K rows x 128 bf16], MN-major: two 64-column boxes
-    static constexpr int kStage = kA + kB;
+struct DgradShape {                              // the epilogue's; the mainloop's are Conv1x1Shape<kDgBN>'s
     static constexpr int kTile = 2 * kSlab;              // [2 column slabs][128 rows x 64 bf16], 128-byte swizzle
     static constexpr int kMask = kCvBM * kDgBN / 8;      // [128 rows][16 mask bytes]
     static constexpr int kEpi = 2 * kTile + kMask;       // x tile, dy2 tile (then g), mask bytes
-    static constexpr int kP = 2 * kBnSlab;
-    static constexpr int kFixed = 2 * kEpi + 8 * kP * 4 + 8 * kP * 8;
+    // the two epilogue buffers, slab_reduce scratch (float), slab_finish totals (double)
+    static constexpr int kFixed = 2 * kEpi + 8 * Conv1x1Shape<kDgBN>::kP * (4 + 8);
 };
 static_assert(kBnBwdReduceUnroll * kBnRows % kCvBM == 0, "a reduction chunk must be whole tiles");
 static_assert(DgradShape::kEpi % 1024 == 0, "epilogue buffers keep the 1024-byte alignment of the swizzled tiles");
@@ -579,20 +624,20 @@ conv1x1_dgrad_bn_bwd_kernel(const __grid_constant__ CUtensorMap tm_dh, const __g
                             const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_dy2,
                             const __grid_constant__ CUtensorMap tm_mask, const __grid_constant__ CUtensorMap tm_g,
                             const DgradArgs a) {
-    using S = DgradShape;
+    using S = Conv1x1Shape<kDgBN>;
+    using E = DgradShape;
     constexpr int kSlabs = kDgBN / kBnSlab;
     extern __shared__ __align__(1024) uint8_t smem[];
     if ((smem_u32(smem) & 1023u) != 0u) __trap();
     const int NS = a.stages;
     uint8_t* ring = smem;                                          // NS x (dH slab, w slab)
-    uint8_t* epi = ring + (size_t)NS * S::kStage;                  // [2] x (x tile, dy2 / g tile, mask bytes)
-    float* red = reinterpret_cast<float*>(epi + 2 * S::kEpi);      // [8 warps][kP]
+    uint8_t* epi = ring + (size_t)NS * S::kStage;
+    float* red = reinterpret_cast<float*>(epi + 2 * E::kEpi);      // [8 warps][kP]
     double* tot = reinterpret_cast<double*>(red + 8 * S::kP);      // [8 warps][kP]
     uint64_t* full = reinterpret_cast<uint64_t*>(tot + 8 * S::kP);
     uint64_t* empty = full + NS;
-    uint64_t* efull = empty + NS;
-    uint64_t* eempty = efull + 2;
-    int* last = reinterpret_cast<int*>(eempty + 2);
+    const EpiRing<E::kEpi> er{epi, empty + NS};                    // [2] x (x tile, dy2 / g tile, mask bytes)
+    int* last = reinterpret_cast<int*>(er.bar + 4);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nb = blockIdx.x, r = blockIdx.y;
@@ -608,7 +653,7 @@ conv1x1_dgrad_bn_bwd_kernel(const __grid_constant__ CUtensorMap tm_dh, const __g
         tma_prefetch_desc(&tm_mask);
         tma_prefetch_desc(&tm_g);
         for (int s = 0; s < NS; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
-        for (int b = 0; b < 2; ++b) { mbar_init(&efull[b], 1); mbar_init(&eempty[b], kBnThreads); }
+        er.init();
         fence_mbar_init();
     }
     __syncthreads();
@@ -620,26 +665,16 @@ conv1x1_dgrad_bn_bwd_kernel(const __grid_constant__ CUtensorMap tm_dh, const __g
             int st = 0;
             uint32_t ph = 0;
             for (int it = 0; it < t1 - t0; ++it) {
-                const int tile = t0 + it, eb = it & 1;
-                const int row0 = tile * kCvBM;
-                mbar_wait(&eempty[eb], ((it >> 1) & 1) ^ 1u);
-                mbar_arrive_expect_tx(&efull[eb], (uint32_t)S::kEpi);  // OOB rows count too (zero-filled)
-                uint8_t* e = epi + eb * S::kEpi;
+                const int tile = t0 + it, row0 = tile * kCvBM;
+                uint8_t* e = er.tile(it);
+                er.acquire(it);
 #pragma unroll
                 for (int s = 0; s < kSlabs; ++s) {
-                    tma_load_2d(&tm_x, &efull[eb], e + s * kSlab, nb * kDgBN + s * 64, row0);
-                    tma_load_2d(&tm_dy2, &efull[eb], e + S::kTile + s * kSlab, nb * kDgBN + s * 64, row0);
+                    tma_load_2d(&tm_x, er.full(it), e + s * kSlab, nb * kDgBN + s * 64, row0);
+                    tma_load_2d(&tm_dy2, er.full(it), e + E::kTile + s * kSlab, nb * kDgBN + s * 64, row0);
                 }
-                tma_load_2d(&tm_mask, &efull[eb], e + 2 * S::kTile, nb * (kDgBN / 8), row0);
-                for (int kc = 0; kc < ksteps; ++kc) {
-                    mbar_wait(&empty[st], ph ^ 1u);
-                    mbar_arrive_expect_tx(&full[st], (uint32_t)S::kStage);
-                    uint8_t* s = ring + (size_t)st * S::kStage;
-                    tma_load_2d(&tm_dh, &full[st], s, kc * 64, row0);
-                    tma_load_2d(&tm_w, &full[st], s + S::kA, nb * kDgBN, kc * 64);
-                    tma_load_2d(&tm_w, &full[st], s + S::kA + S::kB / 2, nb * kDgBN + 64, kc * 64);
-                    if (++st == NS) { st = 0; ph ^= 1u; }
-                }
+                tma_load_2d(&tm_mask, er.full(it), e + 2 * E::kTile, nb * (kDgBN / 8), row0);
+                conv1x1_load_tile<kDgBN, true>(&tm_dh, &tm_w, ring, full, empty, NS, st, ph, tile, nb, ksteps);
             }
         }
         return;
@@ -650,9 +685,6 @@ conv1x1_dgrad_bn_bwd_kernel(const __grid_constant__ CUtensorMap tm_dh, const __g
     const int rloc = wg * 64 + (warp & 3) * 16 + (lane >> 2);    // tile rows rloc and rloc + 8
     const int ccol = 2 * (lane & 3);                              // first of this thread's two columns per 8
     const int v = threadIdx.x & (kBnLanes - 1), rl = threadIdx.x >> 3;   // bn_bwd_reduce_kernel's thread layout
-    const uint64_t a_desc0 = make_sw128_desc(smem_u32(ring + wg * 64 * 128), 16, 1024);
-    const uint64_t b_desc0 = make_sw128_desc(smem_u32(ring + S::kA), S::kB / 2, 1024);
-    constexpr uint64_t kStageUnits = S::kStage >> 4;
     float acc[kDgBN / 2];
     float sacc[kSlabs][16];                                       // per slab: 8 sums of g, 8 of g (x - mean)
     float mu[kSlabs][8];
@@ -666,37 +698,21 @@ conv1x1_dgrad_bn_bwd_kernel(const __grid_constant__ CUtensorMap tm_dh, const __g
     int st = 0;
     uint32_t ph = 0;
     for (int it = 0; it < t1 - t0; ++it) {
-        const int tile = t0 + it, eb = it & 1;
-        int prev = 0;
-        for (int kc = 0; kc < ksteps; ++kc) {
-            mbar_wait(&full[st], ph);
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-                wgmma_ss_tb<kDgBN>(acc, a_desc0 + st * kStageUnits + 2 * k, b_desc0 + st * kStageUnits + 128 * k,
-                                   (kc | k) != 0);
-            wgmma_commit();
-            wgmma_wait<1>();                                      // the previous chunk's wgmmas have completed
-            if (kc > 0 && t == 0) mbar_arrive(&empty[prev]);
-            prev = st;
-            if (++st == NS) { st = 0; ph ^= 1u; }
-        }
-        wgmma_wait<0>();
-        reg_fence(acc);
-        if (t == 0) mbar_arrive(&empty[prev]);
+        const int tile = t0 + it;
+        conv1x1_mma_tile<kDgBN, true>(acc, ring, wg, full, empty, NS, st, ph, ksteps, t);
 
         // ---- epilogue: g = mask . bf16(bf16(dX) + dy2), in place over dy2 -> TMA store; the sums from the staged tile
-        uint8_t* e = epi + eb * S::kEpi;
-        uint8_t* gt = e + S::kTile;
-        const uint8_t* mt = e + 2 * S::kTile;
-        mbar_wait(&efull[eb], (it >> 1) & 1);
+        uint8_t* e = er.tile(it);
+        uint8_t* gt = e + E::kTile;
+        const uint8_t* mt = e + 2 * E::kTile;
+        er.wait(it);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             const int row = rloc + 8 * h;
 #pragma unroll
             for (int j = 0; j < kDgBN / 8; ++j) {
-                __nv_bfloat162* p = reinterpret_cast<__nv_bfloat162*>(gt + (j >> 3) * kSlab + row * 128 +
-                                                                      (((j & 7) ^ (row & 7)) << 4) + (lane & 3) * 4);
+                __nv_bfloat162* p = reinterpret_cast<__nv_bfloat162*>(gt + (j >> 3) * kSlab + sw128_offset(row, j & 7) +
+                                                                      (lane & 3) * 4);
                 const float2 d2 = __bfloat1622float2(*p);
                 const unsigned int bits = (unsigned int)mt[row * (kDgBN / 8) + j] >> ccol;
                 const float d0 = __bfloat162float(__float2bfloat16_rn(acc[4 * j + 2 * h]));
@@ -707,7 +723,7 @@ conv1x1_dgrad_bn_bwd_kernel(const __grid_constant__ CUtensorMap tm_dh, const __g
             }
         }
         fence_proxy_async();                                      // generic smem writes -> visible to the TMA store
-        named_bar_sync(3, kBnThreads);                            // the whole tile staged
+        consumer_sync();                                          // the whole tile staged
         if (threadIdx.x == 0) {
 #pragma unroll
             for (int s = 0; s < kSlabs; ++s) tma_store_2d(&tm_g, gt + s * kSlab, nb * kDgBN + s * 64, tile * kCvBM);
@@ -717,7 +733,7 @@ conv1x1_dgrad_bn_bwd_kernel(const __grid_constant__ CUtensorMap tm_dh, const __g
         for (int p = 0; p < kCvBM / kBnRows; ++p) {
             const int row = p * kBnRows + rl;
             if (tile * kCvBM + row < a.M) {
-                const int off = row * 128 + ((v ^ (row & 7)) << 4);
+                const int off = sw128_offset(row, v);
 #pragma unroll
                 for (int s = 0; s < kSlabs; ++s) {
                     float g[8], f[8];
@@ -731,38 +747,13 @@ conv1x1_dgrad_bn_bwd_kernel(const __grid_constant__ CUtensorMap tm_dh, const __g
                 }
             }
         }
-        if (threadIdx.x == 0) bulk_wait_read<0>();               // the store has read g out of the buffer
-        mbar_arrive(&eempty[eb]);
+        er.release(it);
     }
     if (threadIdx.x == 0) bulk_wait<0>();
 
-    // ---- bn_bwd_reduce_kernel's partials and finish, slab by slab
-#pragma unroll
-    for (int s = 0; s < kSlabs; ++s) {
-        const int gs = nb * kSlabs + s;
-        const float part = slab_reduce<2>(sacc[s], red, ConsumerSync());
-        if (slab_finish<2>(part, a.partial, a.counters + gs, gs, r, a.R, tot, last, ConsumerSync())) {
-            if (threadIdx.x < kBnSlab)
-                bn_bwd_channel<2>(tot, threadIdx.x, gs * kBnSlab + threadIdx.x, a.invstd, a.dbeta, a.dgamma, nullptr,
-                                  nullptr, nullptr);
-        }
-        named_bar_sync(3, kBnThreads);                            // red / tot are reused by the next slab
-    }
-}
-
-// [rows, cols] uint8 row-major tensor (the mask bytes), box = [box_rows, 16 bytes], no swizzle, OOB -> zeros
-static bool make_tmap_u8(CUtensorMap* m, const void* base, int rows, int cols, int box_rows) {
-    EncodeTiledFn fn = get_encode_fn();
-    if (!fn) { set_error("cuTensorMapEncodeTiled entry point not available"); return false; }
-    cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-    cuuint64_t strides[1] = {(cuuint64_t)cols};
-    cuuint32_t box[2] = {16u, (cuuint32_t)box_rows};
-    cuuint32_t estr[2] = {1u, 1u};
-    CUresult res = fn(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), dims, strides, box, estr,
-                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (res != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (CUresult %d)", (int)res); return false; }
-    return true;
+    conv1x1_slabs_finish(sacc, red, tot, last, a.partial, a.counters, nb, r, a.R, [&](int j, int, int c) {
+        bn_bwd_channel<2>(tot, j, c, a.invstd, a.dbeta, a.dgamma, nullptr, nullptr, nullptr);
+    });
 }
 
 // Cin is the BatchNorm's C (a power of two in [128, 2048]); Cout the GEMM's K
@@ -775,42 +766,27 @@ cudaError_t launch_conv1x1_dgrad_bn_bwd(const void* dh, const void* w, void* g, 
                                         const void* x, const void* mask, const void* dy2, const BnLayer& bn, void* ws,
                                         cudaStream_t stream) {
     if (!conv1x1_dgrad_shape_ok(M, Cin, Cout)) return cudaErrorNotSupported;
-    using S = DgradShape;
     DgradArgs a{};
     a.M = (int)M; a.K = Cout;
     a.m_tiles = (int)((M + kCvBM - 1) / kCvBM);
-    long long passes = 0, ppc = 0;
-    bn_bwd_reduce_plan(M, Cin, &passes, &ppc, &a.R);       // bn_bwd_reduce_kernel's row chunks
-    a.ppc = (int)(ppc * kBnRows / kCvBM);
+    a.ppc = tiles_per_cta(bn_bwd_reduce_plan, M, Cin, &a.R);   // bn_bwd_reduce_kernel's row chunks
     const int slices = Cin / kDgBN, slabs = Cin / kBnSlab;
     if ((long long)slabs * a.R > kCvMaxPartials) return cudaErrorNotSupported;
-    constexpr int kBarBytes = 256;
-    int stages = (kSmemBudget - S::kFixed - kBarBytes) / S::kStage;
-    if (stages > 8) stages = 8;
-    if (stages < 2) return cudaErrorNotSupported;
-    a.stages = stages;
-    const int smem = stages * S::kStage + S::kFixed + kBarBytes;
+    int smem = 0;
+    const cudaError_t e = ring_smem(DgradShape::kFixed, Conv1x1Shape<kDgBN>::kStage, &a.stages, &smem);
+    if (e != cudaSuccess) return e;
     a.counters = static_cast<unsigned int*>(ws);
     a.partial = bn_ws_partials(ws);
     a.mean = bn.save_mean; a.invstd = bn.save_invstd; a.dgamma = bn.dgamma; a.dbeta = bn.dbeta;
     CUtensorMap tm_dh, tm_w, tm_x, tm_dy2, tm_mask, tm_g;
     if (!make_tmap(&tm_dh, dh, (int)M, Cout, kCvBM) || !make_tmap(&tm_w, w, Cout, Cin, 64) ||
         !make_tmap(&tm_x, x, (int)M, Cin, kCvBM) || !make_tmap(&tm_dy2, dy2, (int)M, Cin, kCvBM) ||
-        !make_tmap_u8(&tm_mask, mask, (int)M, Cin / 8, kCvBM) || !make_tmap(&tm_g, g, (int)M, Cin, kCvBM))
+        !encode_tmap(&tm_mask, CU_TENSOR_MAP_DATA_TYPE_UINT8, 1, CU_TENSOR_MAP_SWIZZLE_NONE, mask, (int)M, Cin / 8,
+                     kCvBM, 16) ||                         // the mask bytes: [128 rows x 16 bytes] boxes, not swizzled
+        !make_tmap(&tm_g, g, (int)M, Cin, kCvBM))
         return cudaErrorUnknown;
-    {
-        std::lock_guard<std::mutex> lock(g_kernel_cache_mutex);
-        KernelCache& kc = kernel_cache(2);
-        if (kc.smem_set < smem) {
-            cudaError_t e = cudaFuncSetAttribute(conv1x1_dgrad_bn_bwd_kernel,
-                                                 cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-            if (e != cudaSuccess) return e;
-            kc.smem_set = smem;
-        }
-    }
-    conv1x1_dgrad_bn_bwd_kernel<<<dim3(slices, a.R), kCvThreads, smem, stream>>>(tm_dh, tm_w, tm_x, tm_dy2, tm_mask,
-                                                                                  tm_g, a);
-    return launched();
+    return launch_conv1x1<conv1x1_dgrad_bn_bwd_kernel>(dim3(slices, a.R), smem, stream, tm_dh, tm_w, tm_x, tm_dy2,
+                                                       tm_mask, tm_g, a);
 }
 
 }  // namespace moco

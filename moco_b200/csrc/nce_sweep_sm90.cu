@@ -96,7 +96,7 @@ __device__ __forceinline__ void stage_q(const SweepArgs& a, uint8_t* q_s, int ro
             }
             if (pad) { v0 = v1 = v2 = v3 = 0.f; }          // (0/0 of a padding row must not reach the MMA)
             const __nv_bfloat162 lo = __floats2bfloat162_rn(v0, v1), hi = __floats2bfloat162_rn(v2, v3);
-            uint8_t* dst = q_s + (col0 >> 6) * kQSlab + r * 128 + ((((col0 & 63) >> 3) ^ (r & 7)) << 4) + (col0 & 7) * 2;
+            uint8_t* dst = q_s + (col0 >> 6) * kQSlab + sw128_offset(r, (col0 & 63) >> 3) + (col0 & 7) * 2;
             *reinterpret_cast<uint2*>(dst) = make_uint2(*reinterpret_cast<const uint32_t*>(&lo),
                                                         *reinterpret_cast<const uint32_t*>(&hi));
         } else {                                           // 8 bf16 = one 16-byte swizzle chunk
@@ -119,7 +119,7 @@ __device__ __forceinline__ void stage_q(const SweepArgs& a, uint8_t* q_s, int ro
                 u = *reinterpret_cast<const uint4*>(o2);
             }
             if (pad) u = make_uint4(0u, 0u, 0u, 0u);
-            uint8_t* dst = q_s + (col0 >> 6) * kQSlab + r * 128 + ((((col0 & 63) >> 3) ^ (r & 7)) << 4);
+            uint8_t* dst = q_s + (col0 >> 6) * kQSlab + sw128_offset(r, (col0 & 63) >> 3);
             *reinterpret_cast<uint4*>(dst) = u;
         }
     }
@@ -359,9 +359,8 @@ static cudaError_t launch_kc(const __nv_bfloat16* queue, SweepArgs& a, int* slic
     CUtensorMap tm_queue = {};
     if (!plan_only && !make_tmap(&tm_queue, queue, a.K, KC * 64, S::BN / CL)) return cudaErrorUnknown;
     auto fill = [](SweepArgs& x, int slices) { x.slices = slices; };
-    constexpr int slot = (KC - 1) * 8 + MODE * 2 + (CL - 1);
-    return plan_and_launch(nce_sweep_kernel<KC, MODE, CL>, kernel_cache(slot), kSwThreads, smem, CL, a.mblks,
-                           a.mblks * CL, a.num_tiles, a.n_pad, slices_out, stream, tm_queue, a, fill, true, plan_only);
+    return plan_and_launch<nce_sweep_kernel<KC, MODE, CL>>(kSwThreads, smem, CL, a.mblks, a.mblks * CL, a.num_tiles,
+                                                          a.n_pad, slices_out, stream, tm_queue, a, fill, true, plan_only);
 }
 
 template <int MODE, int CL>

@@ -18,6 +18,10 @@ __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
+// Byte offset of 16-byte chunk `chunk` (8 bf16, < 8) of row `row` in a [rows x 64 bf16] slab in the 128-byte-swizzle
+// layout of TMA and wgmma: rows of 128 bytes, chunk c of row r at position c ^ (r & 7).
+__device__ __forceinline__ int sw128_offset(int row, int chunk) { return row * 128 + ((chunk ^ (row & 7)) << 4); }
+
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -34,19 +38,24 @@ inline EncodeTiledFn get_encode_fn() {
     return fn;
 }
 
-// [rows, C] bf16 row-major tensor, box = [box_rows, 64 elements], 128B swizzle, OOB -> zeros.
-inline bool make_tmap(CUtensorMap* m, const void* base, int rows, int C, int box_rows) {
+// [rows, cols] row-major tensor of `elem`-byte elements, box = [box_rows, box_cols], OOB -> zeros.
+inline bool encode_tmap(CUtensorMap* m, CUtensorMapDataType type, int elem, CUtensorMapSwizzle swizzle,
+                        const void* base, int rows, int cols, int box_rows, int box_cols) {
     EncodeTiledFn fn = get_encode_fn();
     if (!fn) { set_error("cuTensorMapEncodeTiled entry point not available"); return false; }
-    cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)rows};
-    cuuint64_t strides[1] = {(cuuint64_t)C * 2};
-    cuuint32_t box[2] = {64u, (cuuint32_t)box_rows};
+    cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+    cuuint64_t strides[1] = {(cuuint64_t)cols * elem};
+    cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
     cuuint32_t estr[2] = {1u, 1u};
-    CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    CUresult r = fn(m, type, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                    swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (CUresult %d)", (int)r); return false; }
     return true;
+}
+
+// [rows, C] bf16 row-major tensor, box = [box_rows, 64 elements], 128B swizzle, OOB -> zeros.
+inline bool make_tmap(CUtensorMap* m, const void* base, int rows, int C, int box_rows) {
+    return encode_tmap(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, CU_TENSOR_MAP_SWIZZLE_128B, base, rows, C, box_rows, 64);
 }
 
 // Per-kernel launch state: the max-dynamic-smem attribute is set once, and the number of clusters that can be
@@ -57,28 +66,38 @@ struct KernelCache {
     int q_smem = -1, q_cluster = -1, q_result = 0;
 };
 
-// cudaFuncSetAttribute and the occupancy answer are per DEVICE: one cache entry per (device ordinal, kernel slot of
-// this translation unit), all guarded by one mutex (launches from several host threads / several GPUs in one process).
-constexpr int kMaxDevices = 64, kCacheSlots = 32;
+// cudaFuncSetAttribute and the occupancy answer are per DEVICE: one cache entry per (device ordinal, kernel), all
+// guarded by one mutex (launches from several host threads / several GPUs in one process).
+constexpr int kMaxDevices = 64;
 static std::mutex g_kernel_cache_mutex;
-static KernelCache& kernel_cache(int slot) {
-    static KernelCache table[kMaxDevices][kCacheSlots];
+template <auto Kern>
+static KernelCache& kernel_cache() {
+    static KernelCache table[kMaxDevices];
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= kMaxDevices) dev = 0;
-    return table[dev][slot];
+    return table[dev];
 }
 
+// Raises the kernel's max-dynamic-smem attribute to smem unless an earlier launch on this device already did; called
+// under g_kernel_cache_mutex.
 template <typename Kern>
-static cudaError_t prepare_kernel(Kern kern, KernelCache& kc, int threads, int smem, int cluster, int* max_clusters) {
-    if (kc.smem_set < smem) {
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        if (e != cudaSuccess) return e;
-        if (cluster > 1) {
-            e = cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 0);
-            (void)e;
-            cudaGetLastError();
-        }
-        kc.smem_set = smem;
+static cudaError_t set_max_smem(Kern kern, KernelCache& kc, int smem) {
+    if (kc.smem_set >= smem) return cudaSuccess;
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e == cudaSuccess) kc.smem_set = smem;
+    return e;
+}
+
+template <auto Kern>
+static cudaError_t prepare_kernel(int threads, int smem, int cluster, int* max_clusters) {
+    KernelCache& kc = kernel_cache<Kern>();
+    const bool first = kc.smem_set < smem;
+    cudaError_t e = set_max_smem(Kern, kc, smem);
+    if (e != cudaSuccess) return e;
+    if (first && cluster > 1) {
+        e = cudaFuncSetAttribute(Kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 0);
+        (void)e;
+        cudaGetLastError();
     }
     if (kc.q_smem != smem || kc.q_cluster != cluster) {
         cudaLaunchConfig_t cfg = {};
@@ -93,7 +112,7 @@ static cudaError_t prepare_kernel(Kern kern, KernelCache& kc, int threads, int s
         cfg.attrs = attr;
         cfg.numAttrs = 1;
         int n = 0;
-        cudaError_t e = cudaOccupancyMaxActiveClusters(&n, kern, &cfg);
+        e = cudaOccupancyMaxActiveClusters(&n, Kern, &cfg);
         if (e != cudaSuccess) return e;
         kc.q_smem = smem; kc.q_cluster = cluster; kc.q_result = n;
     }
@@ -129,16 +148,15 @@ static cudaError_t launch_cluster(Kern kern, int grid, int threads, int smem, in
 }
 
 // plan + launch one templated kernel instance: `fill(slices)` finalises the argument struct
-template <typename Kern, typename Args, typename Fill>
-static cudaError_t plan_and_launch(Kern kern, KernelCache& kc, int threads, int smem, int cluster, int mgroups,
-                                   int ctas_per_slice, int num_tiles, int n_pad, int* slices_out, cudaStream_t stream,
-                                   const CUtensorMap& tmap, Args& args, Fill fill, bool pdl = false,
-                                   bool plan_only = false) {
+template <auto Kern, typename Args, typename Fill>
+static cudaError_t plan_and_launch(int threads, int smem, int cluster, int mgroups, int ctas_per_slice, int num_tiles,
+                                   int n_pad, int* slices_out, cudaStream_t stream, const CUtensorMap& tmap, Args& args,
+                                   Fill fill, bool pdl = false, bool plan_only = false) {
     int max_clusters = 0;
     cudaError_t e;
     {
         std::lock_guard<std::mutex> lock(g_kernel_cache_mutex);
-        e = prepare_kernel(kern, kc, threads, smem, cluster, &max_clusters);
+        e = prepare_kernel<Kern>(threads, smem, cluster, &max_clusters);
     }
     if (e != cudaSuccess) return e;
     int slices = max_clusters / mgroups;            // one persistent wave
@@ -149,7 +167,7 @@ static cudaError_t plan_and_launch(Kern kern, KernelCache& kc, int threads, int 
     *slices_out = slices;
     if (plan_only) return cudaSuccess;          // the caller only needs the (deterministic) slice count
     fill(args, slices);
-    return launch_cluster(kern, ctas_per_slice * slices, threads, smem, cluster, stream, tmap, args, pdl);
+    return launch_cluster(Kern, ctas_per_slice * slices, threads, smem, cluster, stream, tmap, args, pdl);
 }
 
 }  // namespace moco
