@@ -276,8 +276,9 @@ int moco_ema_update(const void* segs_dev, const int32_t* chunk_prefix_dev, int n
  * Two launches per call (reduction + element-wise pass); deterministic.
  *
  * moco_bn_bwd: dy is the gradient w.r.t. y.  With g = dy masked by the ReLU
- * (mask recomputed from x when has_residual == 0, read from y otherwise -- y may be
- * NULL unless relu && has_residual):  dbeta = sum g,  dgamma = sum g * x^,
+ * (mask recomputed from x when has_residual == 0 as y > 0 of the bf16 value the
+ * forward stores, so a positive value that rounds to zero is off; read from y
+ * otherwise -- y may be NULL unless relu && has_residual):  dbeta = sum g,  dgamma = sum g * x^,
  * dx = gamma * invstd * (g - dbeta / M - x^ * dgamma / M),  dresidual = g (written
  * only when dresidual != NULL).
  * ---------------------------------------------------------------------- */

@@ -16,7 +16,8 @@
 //   bn_apply_kernel      reads x (+ residual), writes y = relu(x^ * gamma + beta (+ r)) 4 (6) B / element
 //   bn_bwd_reduce_kernel reads dy, x (+ y)   -> sum(g), sum(g * x^) = dbeta, dgamma     4 (6) B / element
 //   bn_bwd_apply_kernel  reads dy, x (+ y), writes dx (+ d residual)                    6 (10) B / element
-// where g = dy masked by the ReLU (the mask is recomputed from x when there is no residual, read from y otherwise).
+// where g = dy masked by the ReLU (the mask is recomputed from x when there is no residual -- y > 0 of the bf16 value
+// the forward stores -- and read from y otherwise).
 // A block output's gradient may arrive in two parts (the next block's first convolution and its residual branch):
 // both backward passes then read dy and dy2 and use bf16(dy + dy2), +2 B / element each (kSum, moco_bn_add_relu_bwd2).
 //
@@ -230,9 +231,13 @@ struct BnBwdReduceArgs {
     float* sum_dy_xhat2;             // kShortcut: = the shortcut BN's dgamma
 };
 
+// kMaskFromX: y > 0 of the bf16 value bn_apply_kernel stores (relu_bits' rule), so a positive pre-activation that
+// rounds to zero is off.  bf16 rounds z to zero iff z <= 2^-134, half its smallest subnormal (the tie goes to the even
+// zero); the comparison with that constant needs no register for the rounded value (one more spills the
+// 3-CTA / SM apply kernel).
 __device__ __forceinline__ bool mask_on(int mode, float y, unsigned int bits, int k, float x, float ca, float cb) {
     if (mode == kMaskFromY) return y > 0.f;
-    if (mode == kMaskFromX) return fmaf(x, ca, cb) > 0.f;
+    if (mode == kMaskFromX) return fmaf(x, ca, cb) > 0x1p-134f;
     if (mode == kMaskFromBits) return (bits >> k) & 1u;
     return true;
 }
