@@ -36,7 +36,8 @@ enum {
     MOCO_ERR_INVALID = -1,     /* bad argument (null pointer, size, alignment)          */
     MOCO_ERR_UNSUPPORTED = -2, /* valid but not implemented for this shape/dtype/device */
     MOCO_ERR_WORKSPACE = -3,   /* workspace too small                                    */
-    MOCO_ERR_CUDA = -4         /* a CUDA runtime/driver call failed                      */
+    MOCO_ERR_CUDA = -4,        /* a CUDA runtime/driver call failed                      */
+    MOCO_ERR_CAPACITY = -5     /* moco_knn: a query has more candidates than the workspace holds */
 };
 
 enum { MOCO_F32 = 0, MOCO_BF16 = 1 };
@@ -415,6 +416,43 @@ int moco_conv1x1_dgrad_bn_bwd(const void* dh, const void* w, void* g, long long 
 int moco_bn_bwd_apply_given(const void* g, const void* x, const void* x2_or_null, long long M, int C,
                             const moco_bn_layer* bn, const moco_bn_layer* shortcut_or_null, void* dx,
                             void* dx2_or_null, void* stream);
+
+/* ------------------------------------------------------------------------
+ * Weighted k-nearest-neighbour classification against a feature bank (the kNN monitor of instance discrimination,
+ * lemniscate.pytorch's kNN with its weights exp(s / T)), without storing the [Nq, Nb] similarity matrix.
+ *
+ * q: bf16 [Nq, C], 1 <= Nq <= 1024; bank: bf16 [Nb, C], k <= Nb < 2^31 (it may pass 2^32 bytes); C a multiple of 64 in
+ * [64, 2048]; both 16-byte aligned.  labels: int32 [Nb], each in [0, n_classes); n_classes in [1, 65536]; k in
+ * [1, 1024]; inv_T = 1 / T > 0.
+ *   s(i, j) = the fp32 dot product of q_i and bank_j (wgmma, fp32 accumulation in increasing C; exact whenever the
+ *   products' partial sums are exact in fp32).
+ *   N(i) = the first k bank rows under the total order (s descending, j ascending): the result depends on nothing else,
+ *   not on the grid, the workspace or the timing.
+ *   score(i, c) = sum over j in N(i) with labels[j] = c of exp((s(i, j) - s_max(i)) * inv_T), s_max(i) = the largest
+ *   s(i, j); fp32, each class's terms added in N(i)'s order.  Subtracting s_max changes no prediction.
+ *   The predictions are the classes in the order (score descending, class ascending): top5 int32 [Nq, 5] (-1 past
+ *   n_classes), scores5 (nullable) fp32 [Nq, 5] their scores.
+ * nbr_idx / nbr_sim (nullable): int32 / fp32 [Nq, k], N(i) in order and its similarities.  targets (nullable) int32
+ * [Nq] with correct int32 [2]: correct = {#(top5[i][0] == target_i), #(target_i in top5[i])}, over this call.
+ * Outputs may not overlap one another, the inputs or the workspace.  Non-finite features are outside this contract.
+ *
+ * workspace: 256-byte aligned, moco_knn_workspace_bytes(Nq, Nb, capacity) bytes for room for `capacity` candidates
+ * per query (the call uses all it is given, up to Nb); at least capacity = k, else MOCO_ERR_WORKSPACE.  A query's
+ * candidates are the rows with s at least a lower bound on its k-th largest similarity: a few times k for spread
+ * similarities, up to Nb when many rows tie.  When a query has more than the workspace holds, the call returns
+ * MOCO_ERR_CAPACITY; the outputs are then undefined, nothing is truncated, and a call with
+ * moco_knn_workspace_bytes(Nq, Nb, *need_capacity) bytes gives the answer.
+ * need_capacity (HOST): the largest candidate count of any query, also on success.  A label outside [0, n_classes)
+ * among the neighbours is reported after the fact as MOCO_ERR_INVALID.
+ *
+ * Four launches (the two sweeps over the bank on Hopper tensor cores, a threshold kernel, a select-and-vote kernel),
+ * then the call synchronises `stream` to read the candidate counts: it is not graph-capturable.  Needs sm_90.
+ * ---------------------------------------------------------------------- */
+size_t moco_knn_workspace_bytes(int Nq, long long Nb, long long capacity);
+int moco_knn(const void* q, const void* bank, const int32_t* labels, int Nq, long long Nb, int C, int k, float inv_T,
+             int n_classes, const int32_t* targets_or_null, int32_t* top5, float* scores5_or_null,
+             int32_t* nbr_idx_or_null, float* nbr_sim_or_null, int32_t* correct_or_null, void* workspace,
+             size_t workspace_bytes, long long* need_capacity, void* stream);
 
 /* The stem's BatchNorm + ReLU followed by its 3x3 / stride 2 / pad 1 max pooling, without writing the BatchNorm's
  * output: bit-identical to moco_bn_fwd_train (relu = 1, no residual) + moco_maxpool3x3s2_fwd.  The statistics pass,

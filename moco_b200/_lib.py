@@ -23,6 +23,7 @@ ONE_PASS_MAX_INV_T = 25.0          # MOCO_ONE_PASS_MAX_INV_T (include/moco_b200.
 GATHER_AUTO, GATHER_LDG = 0, 1
 BN_STATS_GIVEN, BN_SC_STATS_GIVEN = 1, 2    # moco_bn_fwd_train_given `stats_given` bits
 AUG_GRAY, AUG_FLIP, AUG_JITTER = 1, 2, 4    # moco_aug_crop `flags` bits
+ERR_CAPACITY = -5                  # MOCO_ERR_CAPACITY: moco_knn needs a larger workspace
 
 
 
@@ -101,6 +102,9 @@ SIGNATURES = {
     "moco_bn_relu_maxpool_eval": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "moco_bn_eval_act_avgpool": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
                                          c_void_p, c_void_p, c_void_p]),
+    "moco_knn_workspace_bytes": (c_size_t, [c_int, c_int64, c_int64]),
+    "moco_knn": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int64, c_int, c_int, c_float, c_int, c_void_p, c_void_p,
+                         c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, POINTER(c_int64), c_void_p]),
     "moco_augment_crops": (c_int, [c_void_p, c_size_t, c_void_p, c_int, c_int, c_int, POINTER(c_float), c_void_p, c_int,
                                    c_void_p, c_void_p]),
     "moco_resize_center_crops": (c_int, [c_void_p, c_size_t, c_void_p, c_int, c_int, c_int, POINTER(c_float), c_void_p,

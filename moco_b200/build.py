@@ -8,8 +8,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libmoco_b200.so")
 SOURCES = ["capi.cu", "nce_support.cu", "nce_tail.cu", "nce_sweep_sm90.cu", "queue_shuffle.cu", "ema.cu", "bn_nhwc.cu",
-           "pool_nhwc.cu", "conv1x1_sm90.cu", "augment.cu"]
-HEADERS = ["common.cuh", "bn_reduce.cuh", "sm90_ptx.cuh", "tc_common.cuh", "nce_rows.cuh", os.path.join("..", "..", "include", "moco_b200.h")]
+           "pool_nhwc.cu", "conv1x1_sm90.cu", "knn_sm90.cu", "augment.cu"]
+HEADERS = ["common.cuh", "bn_reduce.cuh", "sm90_ptx.cuh", "tc_common.cuh", "conv1x1_skeleton.cuh", "nce_rows.cuh",
+           os.path.join("..", "..", "include", "moco_b200.h")]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared", "-cudart", "shared",

@@ -721,6 +721,68 @@ int moco_conv1x1_dgrad_bn_bwd(const void* dh, const void* w, void* g, long long 
                        fn);
 }
 
+size_t moco_knn_workspace_bytes(int Nq, long long Nb, long long capacity) {
+    if (Nq < 1 || Nq > kKnnMaxNq || Nb < 1 || Nb >= (1LL << 31) || capacity < 1 || capacity > Nb) return 0;
+    return knn_carve(nullptr, Nq, Nb, capacity).bytes;
+}
+
+int moco_knn(const void* q, const void* bank, const int32_t* labels, int Nq, long long Nb, int C, int k, float inv_T,
+             int n_classes, const int32_t* targets, int32_t* top5, float* scores5, int32_t* nbr_idx, float* nbr_sim,
+             int32_t* correct, void* workspace, size_t workspace_bytes, long long* need_capacity, void* stream_) {
+    g_err[0] = 0;
+    const char* fn = "moco_knn";
+    if (!ptr16(q) || !ptr16(bank) || !labels || !top5 || !workspace || !aligned(workspace, 256) || !need_capacity ||
+        (targets == nullptr) != (correct == nullptr) || !aligned(labels, 4) || !aligned(targets, 4) ||
+        !aligned(top5, 4) || !aligned(scores5, 4) || !aligned(nbr_idx, 4) || !aligned(nbr_sim, 4) ||
+        !aligned(correct, 4))
+        return refuse(fn, MOCO_ERR_INVALID, "bad argument (null / misaligned pointer; targets and correct go together)");
+    if (!(inv_T > 0.f) || !isfinite(inv_T) || n_classes < 1 || n_classes > 65536 || k < 1 || Nb < k)
+        return refuse(fn, MOCO_ERR_INVALID, "needs inv_T > 0 finite, n_classes in [1, 65536] and 1 <= k <= Nb "
+                      "(inv_T=%g n_classes=%d k=%d Nb=%lld)", (double)inv_T, n_classes, k, Nb);
+    if (!knn_shape_ok(Nq, Nb, C, k))
+        return refuse(fn, MOCO_ERR_UNSUPPORTED, "needs 1 <= Nq <= %d, C a multiple of 64 in [64, 2048], k <= 1024 and "
+                      "Nb < 2^31 (Nq=%d C=%d k=%d Nb=%lld)", kKnnMaxNq, Nq, C, k, Nb);
+    // every output apart from the inputs, the workspace and one another
+    struct Buf { const void* p; size_t n; };
+    const Buf in[] = {{q, (size_t)Nq * C * 2}, {bank, (size_t)Nb * C * 2}, {labels, (size_t)Nb * 4},
+                      {targets, (size_t)Nq * 4}, {workspace, workspace_bytes}};
+    const Buf out[] = {{top5, (size_t)Nq * 20}, {scores5, (size_t)Nq * 20}, {nbr_idx, (size_t)Nq * k * 4},
+                       {nbr_sim, (size_t)Nq * k * 4}, {correct, 8}};
+    auto overlap = [](const Buf& a, const Buf& b) {
+        const char *pa = static_cast<const char*>(a.p), *pb = static_cast<const char*>(b.p);
+        return a.p && b.p && pa < pb + b.n && pb < pa + a.n;
+    };
+    for (int i = 0; i < 5; ++i) {
+        for (const Buf& b : in)
+            if (overlap(out[i], b)) return refuse(fn, MOCO_ERR_INVALID, "output %d overlaps an input or the workspace", i);
+        for (int j = 0; j < i; ++j)
+            if (overlap(out[i], out[j])) return refuse(fn, MOCO_ERR_INVALID, "outputs %d and %d overlap", j, i);
+    }
+    KnnWorkspace ws = knn_carve(workspace, Nq, Nb, 0);
+    const size_t need = ws.fixed + (size_t)Nq * k * 8;
+    if (workspace_bytes < need)
+        return refuse(fn, MOCO_ERR_WORKSPACE, "workspace too small (%zu < %zu, a capacity of k candidates per query)",
+                      workspace_bytes, need);
+    long long cap = (long long)((workspace_bytes - ws.fixed) / ((size_t)Nq * 8));
+    if (cap > Nb) cap = Nb;                                // no query has more candidates than the bank has rows
+    ws = knn_carve(workspace, Nq, Nb, cap);
+    const DevInfo d = device_info();
+    if (!d.ok || d.major != 9) return refuse(fn, MOCO_ERR_UNSUPPORTED, "needs an sm_90 device");
+    cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+    const KnnPlan p = {labels, targets, Nq, Nb, C, k, n_classes, inv_T, top5, scores5, nbr_idx, nbr_sim, correct};
+    const int rc = cuda_result(launch_knn(q, bank, p, ws, stream), fn);
+    if (rc != MOCO_OK) return rc;
+    unsigned int status[2] = {0u, 0u};
+    cudaError_t e = cudaMemcpyAsync(status, ws.status, sizeof(status), cudaMemcpyDeviceToHost, stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(stream);
+    if (e != cudaSuccess) return cuda_result(e, fn);
+    *need_capacity = status[0];                            // the largest candidate count of any query
+    if (status[1]) return refuse(fn, MOCO_ERR_INVALID, "a neighbour's label is outside [0, %d)", n_classes);
+    if (status[0] > (unsigned long long)cap)
+        return refuse(fn, MOCO_ERR_CAPACITY, "a query has %u candidates, the workspace holds %lld", status[0], cap);
+    return MOCO_OK;
+}
+
 int moco_bn_bwd_apply_given(const void* g, const void* x, const void* x2, long long M, int C, const moco_bn_layer* bn,
                             const moco_bn_layer* shortcut, void* dx, void* dx2, void* stream_) {
     g_err[0] = 0;

@@ -186,6 +186,33 @@ cudaError_t launch_conv1x1_bn_add_relu(const void* x, const void* w, const void*
 cudaError_t launch_conv1x1_dgrad_bn_bwd(const void* dh, const void* w, void* g, long long M, int Cin, int Cout,
                                         const void* x, const void* mask, const void* dy2, const BnLayer& bn, void* ws,
                                         cudaStream_t stream);
+// kNN classification against a feature bank (knn_sm90.cu, moco_knn)
+constexpr int kKnnMaxNq = 1024;
+struct KnnWorkspace {
+    unsigned int* status;          // [0] the largest candidate count, [1] a label outside [0, n_classes)
+    unsigned int* count;           // [Nq] candidates per query
+    float* thresh;                 // [Nq] the sweep-2 threshold
+    float* slice_max;              // [Nq][n_slices] the sweep-1 slice maxima
+    unsigned long long* cand;      // [Nq][cap] candidate keys
+    long long n_slices, cap;
+    size_t fixed, bytes;           // fixed: everything but the candidate lists
+};
+struct KnnPlan {
+    const int* labels;
+    const int* targets;            // nullable
+    int Nq;
+    long long Nb;
+    int C, k, n_classes;
+    float inv_T;
+    int* top5;
+    float* scores5;                // nullable
+    int* nbr_idx;                  // nullable
+    float* nbr_sim;                // nullable
+    int* correct;                  // nullable
+};
+KnnWorkspace knn_carve(void* base, int Nq, long long Nb, long long cap);
+bool knn_shape_ok(int Nq, long long Nb, int C, int k);
+cudaError_t launch_knn(const void* q, const void* bank, const KnnPlan& p, const KnnWorkspace& ws, cudaStream_t stream);
 bool augment_shape_ok(int n_crops, int out_h, int out_w);
 cudaError_t launch_augment(const void* pixels, size_t pixels_bytes, const moco_aug_crop* crops, int n_crops, int out_h,
                            int out_w, const float norm[6], void* dst, int dst_dtype, float* crop_means,
