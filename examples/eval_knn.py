@@ -56,7 +56,7 @@ def main(argv=None):
     from torch.utils.data import DataLoader
     from moco_b200 import augment as A
     from moco_b200 import checkpoint
-    from moco_b200.encoders import from_reference_state_dict, resnet50
+    from moco_b200.encoders import encoder_from_state_dict
     from moco_b200.knn import build_bank, knn_evaluate
     from moco_b200.linear_eval import ShardSampler
 
@@ -69,9 +69,9 @@ def main(argv=None):
     rank = dist.get_rank() if world > 1 else 0
     t0 = time.perf_counter()
 
-    model = resnet50(width=args.model_width).to(dev).to(memory_format=torch.channels_last)
     ckpt = checkpoint.load(args.pretrained)
-    model.load_state_dict(from_reference_state_dict(ckpt["model"]))
+    model = encoder_from_state_dict(ckpt["model"], width=args.model_width)   # with the MLP head an --mlp run trained
+    model = model.to(dev).to(memory_format=torch.channels_last)
     model.freeze()
     if rank == 0:
         print(f"loaded {args.pretrained} (epoch {ckpt.get('epoch', '?')})", flush=True)

@@ -106,7 +106,7 @@ def main(argv=None):
     import torch
     import torch.distributed as dist
     from moco_b200 import checkpoint
-    from moco_b200.encoders import from_reference_state_dict, resnet50
+    from moco_b200.encoders import encoder_from_state_dict, resnet50
     from moco_b200.linear_eval import LinearClassifierResNet
 
     world = int(os.environ.get("WORLD_SIZE", 1))
@@ -118,12 +118,14 @@ def main(argv=None):
     rank = dist.get_rank() if world > 1 else 0
     torch.manual_seed(args.rng_seed)                                                      # eval.py:81-82
 
-    model = resnet50(width=args.model_width).to(dev).to(memory_format=torch.channels_last)
     if args.pretrained:                                                                  # eval.py:149-153
         ckpt = checkpoint.load(args.pretrained)
-        model.load_state_dict(from_reference_state_dict(ckpt["model"]))
+        model = encoder_from_state_dict(ckpt["model"], width=args.model_width)   # an MLP head is loaded, not read
         if rank == 0:
             print(f"loaded {args.pretrained} (epoch {ckpt.get('epoch', '?')})", flush=True)
+    else:
+        model = resnet50(width=args.model_width)
+    model = model.to(dev).to(memory_format=torch.channels_last)
     model.freeze()
     if args.data_dir:
         res = run_data(args, model, dev, rank, world)

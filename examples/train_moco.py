@@ -61,7 +61,11 @@ def parse_args(argv=None):
                     help="ImageFolder root with train/ (train.py:94); decoded by the workers, augmented on the GPU "
                          "(moco_b200/augment.py).  Without it the inputs are synthetic.")
     ap.add_argument("--crop", type=float, default=0.08, help="minimum crop scale (train.py: --crop)")
-    ap.add_argument("--aug", default="CJ", choices=["NULL", "CJ"], help="train.py: --aug")
+    ap.add_argument("--aug", default="CJ", choices=["NULL", "CJ", "V2"],
+                    help="train.py: --aug; V2 is MoCo v2's aug-plus (colour jitter 0.8, grayscale after it, Gaussian "
+                         "blur 0.5; moco_b200/augment.py)")
+    ap.add_argument("--mlp", action="store_true",
+                    help="MoCo v2's projection head: fc is Linear(C, C) -> ReLU -> Linear(C, 128)")
     ap.add_argument("--num-workers", type=int, default=4, help="DataLoader workers per GPU (train.py: --num-workers)")
     # the recipe (train.py's flags and defaults)
     ap.add_argument("--epochs", type=int, default=200)
@@ -142,8 +146,8 @@ def main(argv=None):
 
     torch.manual_seed(0)
     ctor = getattr(encoders, args.arch)
-    model = ctor(low_dim=128, width=args.model_width).to(dev).to(memory_format=torch.channels_last)
-    model_ema = ctor(low_dim=128, width=args.model_width).to(dev).to(memory_format=torch.channels_last)
+    model = ctor(low_dim=128, width=args.model_width, mlp=args.mlp).to(dev).to(memory_format=torch.channels_last)
+    model_ema = ctor(low_dim=128, width=args.model_width, mlp=args.mlp).to(dev).to(memory_format=torch.channels_last)
     moment_update(model, model_ema, 0)                                                    # train.py:133
     contrast = MemoryMoCo(128, args.nce_k, args.nce_t, persist_index=args.persist_index,
                           device_index=args.graph_tail).to(dev)                          # train.py:181
@@ -208,10 +212,15 @@ def run_recipe(args, dev, rank, world):
     if n_iter == 0:
         raise ValueError(f"{len(loader.dataset)} training images give no full batch of {args.batch_size} per rank")
 
+    ckpt = checkpoint.load(args.resume) if args.resume else None
+    if ckpt is not None and encoders.has_mlp_head(ckpt["model"]) != args.mlp:
+        have = not args.mlp
+        raise ValueError(f"--resume {args.resume}: its encoder has {'the' if have else 'no'} MLP head; resume it "
+                         f"{'with' if have else 'without'} --mlp")
     torch.manual_seed(args.rng_seed)
     ctor = getattr(encoders, args.arch)
-    model = ctor(low_dim=128, width=args.model_width).to(dev).to(memory_format=torch.channels_last)
-    model_ema = ctor(low_dim=128, width=args.model_width).to(dev).to(memory_format=torch.channels_last)
+    model = ctor(low_dim=128, width=args.model_width, mlp=args.mlp).to(dev).to(memory_format=torch.channels_last)
+    model_ema = ctor(low_dim=128, width=args.model_width, mlp=args.mlp).to(dev).to(memory_format=torch.channels_last)
     moment_update(model, model_ema, 0)                                                    # train.py:133
     contrast = MemoryMoCo(128, args.nce_k, args.nce_t, persist_index=args.persist_index,
                           device_index=args.graph_tail).to(dev)                          # train.py:181
@@ -220,8 +229,8 @@ def run_recipe(args, dev, rank, world):
     scheduler = get_scheduler(opt, n_iter, args.epochs, args.lr_scheduler, args.warmup_epoch,
                               args.warmup_multiplier, args.lr_decay_epochs, args.lr_decay_rate)
     start_epoch = 1
-    if args.resume:
-        start_epoch = checkpoint.restore(checkpoint.load(args.resume), model, model_ema, contrast, opt)
+    if ckpt is not None:
+        start_epoch = checkpoint.restore(ckpt, model, model_ema, contrast, opt)
         scheduler.load_state_dict({"last_epoch": (start_epoch - 1) * n_iter})
         if rank == 0:
             print(f"resumed {args.resume}: epoch {start_epoch}, lr {opt.param_groups[0]['lr']:.6g}", flush=True)

@@ -29,7 +29,8 @@ extern "C" {
 #endif
 
 #define MOCO_B200_ABI_VERSION 3 /* 3: + moco_bn_*, moco_maxpool3x3s2_*, moco_crop_s2d_bf16, moco_conv1x1_*,
-                                    moco_augment_crops, moco_launch_count, moco_resize_center_crops (additive) */
+                                    moco_augment_crops, moco_launch_count, moco_resize_center_crops,
+                                    moco_augment_crops_blur (additive) */
 
 enum {
     MOCO_OK = 0,
@@ -595,6 +596,52 @@ typedef struct moco_aug_crop {
 
 int moco_augment_crops(const void* pixels, size_t pixels_bytes, const moco_aug_crop* crops, int n_crops, int out_h,
                        int out_w, const float* norm_host, void* dst, int dst_dtype, float* crop_means, void* stream);
+
+/* ------------------------------------------------------------------------
+ * The MoCo v2 augmentation ("aug-plus"): RandomResizedCrop -> RandomApply(ColorJitter, 0.8) -> RandomGrayscale ->
+ * RandomApply(GaussianBlur(ksize, sigma), 0.5) -> RandomHorizontalFlip -> Normalize, in the conventions of
+ * moco_augment_crops above.  Each record is a moco_aug_crop followed by two switches and the blur's weights:
+ *   1. the resample, as moco_augment_crops;
+ *   2. rgb_to_grayscale when flags has MOCO_AUG_GRAY and gray_after_jitter == 0;
+ *   3. the jitter, as moco_augment_crops (flags MOCO_AUG_JITTER, order, factors);
+ *   4. rgb_to_grayscale when flags has MOCO_AUG_GRAY and gray_after_jitter != 0 (the v2 order);
+ *   5. when blur != 0, torchvision's tensor gaussian_blur with the 1-D kernel k[j] = weights[|j - h|], j = 0 .. 2h,
+ *      h = ksize / 2: reflect padding of h on the crop as it stands after step 4 (row -i is row i, row out_h - 1 + i
+ *      is row out_h - 1 - i; columns likewise), then
+ *          t(y, x)   = sum for j = 0 .. 2h of k[j] * s(reflect(y - h + j), x)     (vertical pass first)
+ *          out(y, x) = sum for j = 0 .. 2h of k[j] * t(y, reflect(x - h + j))     (then the horizontal pass)
+ *      each sum started from 0 and taken in tap order j, every product and addition one fp32 operation rounded to
+ *      nearest.  The blur runs in unflipped coordinates, before the flip;
+ *   6. hflip when flags has MOCO_AUG_FLIP, then Normalize.
+ * The contrast mean is that of moco_augment_crops: the mean grayscale before the contrast op, before any blur.
+ * torchvision's conv2d sums the rounded 2-D products ky[a] * kx[b] in its own order, so the blurred crops, too, agree
+ * with torchvision to fp32 rounding; tests/augment_blur_oracle.py restates this order and the kernels match it bit
+ * for bit.  With blur = 0 and gray_after_jitter = 0 a record computes exactly what moco_augment_crops computes.
+ *
+ * weights: the half kernel kernel1d[h], kernel1d[h + 1], ..., kernel1d[2h], zero past index h.  The caller computes
+ * them on the host with torchvision's _get_gaussian_kernel1d arithmetic (linspace, exp(-0.5 (x / sigma)^2), / sum, in
+ * fp32), which is symmetric bit for bit for an odd ksize; the device evaluates no transcendental function.
+ * ksize: odd, in [3, 31], ksize / 2 < min(out_h, out_w) (reflect padding needs it); one per call.
+ * out_h, out_w in [1, 512]; n_crops in [0, 65535]; a crop at most 1000 * out_w pixels wide.  Anything outside this
+ * envelope is refused before any launch.  crops: DEVICE array, 8-byte aligned.  A malformed record gives unspecified
+ * values but never reads outside the pixel buffer or shared memory: source indices are clamped as in
+ * moco_augment_crops, the two switches are tested against 0 and the weights are only multiplied.
+ *
+ * Three launches, each over all n_crops records: the contrast means; the apply pass of the unblurred crops (8 output
+ * rows per CTA, as moco_augment_crops; a blurred crop's CTAs exit at once); the apply pass of the blurred crops, each
+ * CTA a band of up to 32 output rows at full width that evaluates steps 1-4 for its rows and the h rows either side
+ * into shared memory as fp32 RGB and blurs out of it (an unblurred crop's CTAs exit at once).  Deterministic.
+ * ---------------------------------------------------------------------- */
+typedef struct moco_aug_crop_blur {
+    moco_aug_crop crop;                   /* the moco_aug_crop record, unchanged in meaning              */
+    int32_t gray_after_jitter;            /* 0: grayscale before the jitter (v1), else after it (v2)     */
+    int32_t blur;                         /* 0: no blur                                                  */
+    float weights[16];                    /* the half kernel, kernel1d[h + i]; zero past i = h           */
+} moco_aug_crop_blur;                     /* 128 bytes                                                   */
+
+int moco_augment_crops_blur(const void* pixels, size_t pixels_bytes, const moco_aug_crop_blur* crops, int n_crops,
+                            int out_h, int out_w, int ksize, const float* norm_host, void* dst, int dst_dtype,
+                            float* crop_means, void* stream);
 
 /* ------------------------------------------------------------------------
  * The validation transform of the linear evaluation (eval.py:111-116: Resize(256) -> CenterCrop(224) -> ToTensor ->

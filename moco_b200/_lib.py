@@ -107,6 +107,8 @@ SIGNATURES = {
                          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, POINTER(c_int64), c_void_p]),
     "moco_augment_crops": (c_int, [c_void_p, c_size_t, c_void_p, c_int, c_int, c_int, POINTER(c_float), c_void_p, c_int,
                                    c_void_p, c_void_p]),
+    "moco_augment_crops_blur": (c_int, [c_void_p, c_size_t, c_void_p, c_int, c_int, c_int, c_int, POINTER(c_float),
+                                        c_void_p, c_int, c_void_p, c_void_p]),
     "moco_resize_center_crops": (c_int, [c_void_p, c_size_t, c_void_p, c_int, c_int, c_int, POINTER(c_float), c_void_p,
                                          c_int, c_void_p]),
     "moco_crop_to_nhwc_bf16": (c_int, [c_void_p, c_int, c_int64, c_void_p, c_int, c_int, c_int, c_void_p]),

@@ -14,6 +14,15 @@ Semantics: each crop equals torchvision's TENSOR implementation of the reference
 reference itself runs PIL on uint8, which rounds after the resize and after every jitter op, uses its own grayscale
 weights and rounds the contrast mean to an integer; on the same draws the two differ by about one uint8 level on
 average.
+
+MoCo v2's augmentation (``aug="V2"``: RandomResizedCrop -> RandomApply(ColorJitter(0.4, 0.4, 0.4, 0.1), 0.8) ->
+RandomGrayscale(0.2) -> RandomApply(GaussianBlur, 0.5) -> RandomHorizontalFlip -> Normalize) runs through
+``moco_augment_crops_blur`` on 32-word records.  Its blur is torchvision's tensor ``GaussianBlur(23, (0.1, 2.0))``:
+reflect padding and a fixed 23-tap kernel whose weights the workers compute with torchvision's own arithmetic
+(``gaussian_half_kernel``), with sigma drawn by ``GaussianBlur.get_params`` on the torch RNG.  MoCo v2's own code
+blurs with PIL's ``ImageFilter.GaussianBlur``, an approximation with no fixed kernel size, and draws sigma with
+Python's ``random``; drawing on the torch RNG keeps ``seed_epoch``'s exact resume.  ``reference_crop`` rebuilds the
+blur's kernel from the record's weights (the record holds no sigma), which are torchvision's bits.
 """
 from __future__ import annotations
 
@@ -40,22 +49,58 @@ WORDS = 14
 RESIZED_H, RESIZED_W, WIN_TOP, WIN_LEFT = range(4, 8)
 WIN_WORDS = 8
 
+# one moco_aug_crop_blur record (MoCo v2) as 32 int32 words: the 14 above, the two switches and the half kernel
+GRAY_LATE, BLUR, WEIGHTS = 14, 15, 16
+V2_WORDS = 32
+BLUR_KSIZE = 23                        # MoCo v2's blur as torchvision's tensor GaussianBlur(23, (0.1, 2.0))
+BLUR_SIGMA = (0.1, 2.0)
+AUGS = ("NULL", "CJ", "V2")
+
 _JITTER = T.ColorJitter(0.4, 0.4, 0.4, 0.4)     # train.py:110; its ranges as torchvision stores them
+_JITTER_V2 = T.ColorJitter(0.4, 0.4, 0.4, 0.1)  # MoCo v2's aug-plus
 
 
 def _float_bits(values) -> list[int]:
     return torch.tensor(values, dtype=torch.float32).view(torch.int32).tolist()
 
 
+def gaussian_half_kernel(ksize: int, sigma: float) -> list[float]:
+    """kernel1d[ksize // 2:] of torchvision's _get_gaussian_kernel1d(ksize, sigma, float32, cpu), by the same torch
+    ops, padded with zeros to 16 values: the weights of a moco_aug_crop_blur record."""
+    half = (ksize - 1) * 0.5
+    x = torch.linspace(-half, half, steps=ksize, dtype=torch.float32)
+    pdf = torch.exp(-0.5 * (x / sigma).pow(2))
+    k = pdf / pdf.sum()
+    return k[ksize // 2:].tolist() + [0.0] * (16 - (ksize + 1) // 2)
+
+
 def sample_crop_params(h: int, w: int, scale=(0.08, 1.0), aug: str = "CJ") -> torch.Tensor:
     """The random draws of one crop of an h x w image, made by torchvision's code on the global (or worker) RNG in
     the order the reference's Compose makes them (train.py:98-114): RandomResizedCrop.get_params, then for
     ``aug="CJ"`` the grayscale draw and ColorJitter.get_params, then the flip draw.  Returns the int32 [14] record
-    with src_offset 0."""
-    if aug not in ("CJ", "NULL"):
+    with src_offset 0.  ``aug="V2"`` draws MoCo v2's Compose: RandomResizedCrop.get_params, RandomApply's draw and
+    ColorJitter.get_params only if it applies, the grayscale draw, RandomApply's draw and GaussianBlur.get_params
+    only if it applies, the flip draw; it returns the int32 [32] moco_aug_crop_blur record."""
+    if aug not in AUGS:
         raise NotImplementedError(f"augmentation not supported: {aug}")
     top, left, ch, cw = T.RandomResizedCrop.get_params(torch.empty(1, 1, 1).expand(3, h, w), scale, RATIO)
     flags, order, factors = 0, 0, [1.0, 1.0, 1.0, 0.0]
+    if aug == "V2":
+        if not 0.8 < torch.rand(1):                                                  # RandomApply(p=0.8)
+            fn_idx, b, c, s, hue = T.ColorJitter.get_params(_JITTER_V2.brightness, _JITTER_V2.contrast,
+                                                            _JITTER_V2.saturation, _JITTER_V2.hue)
+            flags |= _lib.AUG_JITTER
+            order = sum(int(op) << (2 * k) for k, op in enumerate(fn_idx.tolist()))
+            factors = [b, c, s, hue]
+        if torch.rand(1) < 0.2:                                                      # RandomGrayscale(p=0.2)
+            flags |= _lib.AUG_GRAY
+        blur, weights = 0, [0.0] * 16
+        if not 0.5 < torch.rand(1):                                                  # RandomApply(p=0.5)
+            blur, weights = 1, gaussian_half_kernel(BLUR_KSIZE, T.GaussianBlur.get_params(*BLUR_SIGMA))
+        if torch.rand(1) < 0.5:                                                      # RandomHorizontalFlip()
+            flags |= _lib.AUG_FLIP
+        return torch.tensor([0, 0, h, w, top, left, ch, cw, flags, order] + _float_bits(factors) + [1, blur] +
+                            _float_bits(weights), dtype=torch.int32)
     if aug == "CJ":
         if torch.rand(1) < 0.2:                                                      # RandomGrayscale(p=0.2)
             flags |= _lib.AUG_GRAY
@@ -98,6 +143,37 @@ def validate_params(params: torch.Tensor, pixels_bytes: int, out_w: int | None =
     bad(jit & ~perm, "jitter order is not a permutation of the four ops")
     bad(~np.isfinite(f).all(axis=1), "non-finite factor")
     bad(jit & ((f[:, :3] < 0).any(axis=1) | (np.abs(f[:, 3]) > 0.5)), "factor out of range")
+
+
+def validate_params_v2(params: torch.Tensor, pixels_bytes: int, out_w: int | None = None,
+                       ksize: int = BLUR_KSIZE) -> None:
+    """Raise ValueError unless every record of the int32 [n, 32] ``params`` passes ``validate_params`` on its first
+    14 words, has 0 or 1 as its two switches, and weights that are finite, in [0, 1] and zero past ksize // 2."""
+    p = np.asarray(params.detach().cpu(), dtype=np.int32)
+    if p.ndim != 2 or p.shape[1] != V2_WORDS:
+        raise ValueError(f"crop parameters must be int32 [n, {V2_WORDS}], got {tuple(p.shape)}")
+    if not (3 <= ksize <= 31 and ksize % 2):
+        raise ValueError(f"crop parameters: the blur's ksize must be odd and in [3, 31], got {ksize}")
+    validate_params(torch.from_numpy(np.ascontiguousarray(p[:, :WORDS])), pixels_bytes, out_w)
+    wts = p[:, WEIGHTS:].copy().view(np.float32)
+
+    def bad(mask, what):
+        if mask.any():
+            raise ValueError(f"crop parameters: {what} (record {int(np.flatnonzero(mask)[0])})")
+
+    bad((p[:, GRAY_LATE] != 0) & (p[:, GRAY_LATE] != 1), "gray_after_jitter is not 0 or 1")
+    bad((p[:, BLUR] != 0) & (p[:, BLUR] != 1), "blur is not 0 or 1")
+    bad(~np.isfinite(wts).all(axis=1), "non-finite blur weight")
+    bad(((wts < 0) | (wts > 1)).any(axis=1), "blur weight outside [0, 1]")
+    bad((wts[:, ksize // 2 + 1:] != 0).any(axis=1), f"blur weight past ksize // 2 = {ksize // 2}")
+
+
+def _validate_records(params, pixels_bytes, out_w=None):
+    """validate_params or validate_params_v2, by the records' width."""
+    if params.dim() == 2 and params.shape[1] == V2_WORDS:
+        validate_params_v2(params, pixels_bytes, out_w)
+    else:
+        validate_params(params, pixels_bytes, out_w)
 
 
 def resize_window_params(h: int, w: int, resize: int = 256, out: int = 224) -> torch.Tensor:
@@ -156,11 +232,11 @@ def pack_images(images, records) -> tuple[torch.Tensor, torch.Tensor]:
 
 class ImageFolderTwoCrop(torchvision.datasets.ImageFolder):
     """moco/dataset.py's ImageFolderInstance(two_crop=True) with train.py's transform, minus the pixel work: an item
-    is (decoded uint8 HWC image, int32 [2, 14] parameters of its two crops, target).  Use ``collate_fn`` as the
-    DataLoader's collate_fn and ``augment_two_crop`` on what it yields."""
+    is (decoded uint8 HWC image, int32 [2, 14] parameters of its two crops, target), [2, 32] for ``aug="V2"``.  Use
+    ``collate_fn`` as the DataLoader's collate_fn and ``augment_two_crop`` on what it yields."""
 
     def __init__(self, root, scale=(0.08, 1.0), aug: str = "CJ"):
-        if aug not in ("CJ", "NULL"):
+        if aug not in AUGS:
             raise NotImplementedError(f"augmentation not supported: {aug}")
         super().__init__(root)
         self.scale = tuple(scale)
@@ -179,7 +255,7 @@ class ImageFolderTwoCrop(torchvision.datasets.ImageFolder):
         """[(hwc, params, target)] -> (uint8 [sum of h*w*3] packed pixels, int32 [2N, 14] params with each image's
         byte offset filled in, int64 [N] targets).  DataLoader(pin_memory=True) pins all three."""
         pixels, params = pack_images([it[0] for it in items], [it[1] for it in items])
-        validate_params(params, pixels.numel())
+        _validate_records(params, pixels.numel())
         return pixels, params, torch.tensor([it[2] for it in items], dtype=torch.int64)
 
 
@@ -234,10 +310,11 @@ def _device(device, what):
 def augment_crops(batch, out_size=224, mean=MEAN, std=STD, dtype=torch.bfloat16, device=None) -> torch.Tensor:
     """(pixels, params, ...) with int32 [n, 14] crop records -> [n, 3, H, W], one crop per record, computed on
     ``device`` (default: the current CUDA device) by one C call (moco_augment_crops).  The pixels and records are
-    copied with non_blocking=True (asynchronous from pinned memory)."""
+    copied with non_blocking=True (asynchronous from pinned memory).  int32 [n, 32] records (``aug="V2"``) go to
+    moco_augment_crops_blur with the blur's kernel size BLUR_KSIZE."""
     pixels, params = batch[0], batch[1]
     out_h, out_w = (out_size, out_size) if isinstance(out_size, int) else tuple(out_size)
-    validate_params(params, pixels.numel(), out_w)
+    _validate_records(params, pixels.numel(), out_w)
     dev = _device(device, "augment_crops")
     if pixels.dtype != torch.uint8:
         raise TypeError("augment_crops: pixels must be uint8")
@@ -249,9 +326,14 @@ def augment_crops(batch, out_size=224, mean=MEAN, std=STD, dtype=torch.bfloat16,
     norm = (ctypes.c_float * 6)(*mean, *std)
     with torch.cuda.device(dev):
         lib = _lib.load()
-        _lib.check(lib.moco_augment_crops(pix.data_ptr(), pix.numel(), prm.data_ptr(), n, out_h, out_w, norm,
-                                          out.data_ptr(), _lib.dtype_code(out), means.data_ptr(), _lib.cur_stream()),
-                   "moco_augment_crops")
+        if prm.shape[1] == V2_WORDS:
+            _lib.check(lib.moco_augment_crops_blur(pix.data_ptr(), pix.numel(), prm.data_ptr(), n, out_h, out_w,
+                                                   BLUR_KSIZE, norm, out.data_ptr(), _lib.dtype_code(out),
+                                                   means.data_ptr(), _lib.cur_stream()), "moco_augment_crops_blur")
+        else:
+            _lib.check(lib.moco_augment_crops(pix.data_ptr(), pix.numel(), prm.data_ptr(), n, out_h, out_w, norm,
+                                              out.data_ptr(), _lib.dtype_code(out), means.data_ptr(),
+                                              _lib.cur_stream()), "moco_augment_crops")
     return out
 
 
@@ -321,29 +403,47 @@ def resize_center_crops(batch, resize=256, out=224, mean=MEAN, std=STD, dtype=to
     return dst
 
 
-def reference_crop(hwc_uint8: torch.Tensor, record, out_size=224, mean=MEAN, std=STD) -> torch.Tensor:
+def reference_crop(hwc_uint8: torch.Tensor, record, out_size=224, mean=MEAN, std=STD,
+                   ksize: int = BLUR_KSIZE) -> torch.Tensor:
     """What the kernel computes for one crop, with torchvision's functional tensor ops on the CPU:
-    [3, H, W] fp32 from a uint8 HWC image and one int32 [14] record (train.py:106-114 with the record's draws)."""
+    [3, H, W] fp32 from a uint8 HWC image and one int32 [14] record (train.py:106-114 with the record's draws).
+    A 32-word record is MoCo v2's: the grayscale after the jitter when gray_after_jitter is set, and with blur set
+    torchvision's tensor gaussian_blur of size ``ksize`` with the kernel rebuilt from the record's weights."""
     r = [int(v) for v in record]
-    f = torch.tensor(r[BRIGHTNESS:], dtype=torch.int32).view(torch.float32).tolist()
+    f = torch.tensor(r[BRIGHTNESS:WORDS], dtype=torch.int32).view(torch.float32).tolist()
+    v2 = len(r) == V2_WORDS
+    gray_late = v2 and r[GRAY_LATE] != 0
     out_hw = [out_size, out_size] if isinstance(out_size, int) else list(out_size)
     x = hwc_uint8.permute(2, 0, 1).float() / 255
     x = TF.resized_crop(x, r[TOP], r[LEFT], r[HEIGHT], r[WIDTH], out_hw, antialias=True)
-    if r[FLAGS] & _lib.AUG_GRAY:
+    if r[FLAGS] & _lib.AUG_GRAY and not gray_late:
         x = TF.rgb_to_grayscale(x, 3)
     if r[FLAGS] & _lib.AUG_JITTER:
         ops = (TF.adjust_brightness, TF.adjust_contrast, TF.adjust_saturation, TF.adjust_hue)
         for k in range(4):
             op = (r[ORDER] >> (2 * k)) & 3
             x = ops[op](x, f[op])
+    if r[FLAGS] & _lib.AUG_GRAY and gray_late:
+        x = TF.rgb_to_grayscale(x, 3)
+    if v2 and r[BLUR]:
+        half = torch.tensor(r[WEIGHTS:], dtype=torch.int32).view(torch.float32)[:ksize // 2 + 1]
+        k1d = torch.cat([half.flip(0)[:-1], half])
+        k2d = torch.mm(k1d[:, None], k1d[None, :]).expand(3, 1, ksize, ksize)
+        x = torch.nn.functional.pad(x[None], [ksize // 2] * 4, mode="reflect")
+        x = torch.nn.functional.conv2d(x, k2d, groups=3)[0]
     if r[FLAGS] & _lib.AUG_FLIP:
         x = TF.hflip(x)
     return TF.normalize(x, list(mean), list(std))
 
 
 def reference_compose(aug: str = "CJ", scale=(0.08, 1.0), out_size=224):
-    """train.py:98-114's transform as tensor ops on a float [3, h, w] image in [0, 1] (ToTensor already applied)."""
-    if aug == "NULL":
+    """train.py:98-114's transform as tensor ops on a float [3, h, w] image in [0, 1] (ToTensor already applied);
+    ``aug="V2"`` MoCo v2's, with torchvision's tensor GaussianBlur(23, (0.1, 2.0))."""
+    if aug == "V2":
+        ts = [T.RandomResizedCrop(out_size, scale=scale), T.RandomApply([T.ColorJitter(0.4, 0.4, 0.4, 0.1)], p=0.8),
+              T.RandomGrayscale(p=0.2), T.RandomApply([T.GaussianBlur(BLUR_KSIZE, BLUR_SIGMA)], p=0.5),
+              T.RandomHorizontalFlip()]
+    elif aug == "NULL":
         ts = [T.RandomResizedCrop(out_size, scale=scale), T.RandomHorizontalFlip()]
     else:
         ts = [T.RandomResizedCrop(out_size, scale=scale), T.RandomGrayscale(p=0.2), T.ColorJitter(0.4, 0.4, 0.4, 0.4),

@@ -546,6 +546,29 @@ int moco_augment_crops(const void* pixels, size_t pixels_bytes, const moco_aug_c
                        "augment kernels");
 }
 
+int moco_augment_crops_blur(const void* pixels, size_t pixels_bytes, const moco_aug_crop_blur* crops, int n_crops,
+                            int out_h, int out_w, int ksize, const float* norm, void* dst, int dst_dtype,
+                            float* crop_means, void* stream_) {
+    g_err[0] = 0;
+    static_assert(sizeof(moco_aug_crop_blur) == 128, "moco_aug_crop_blur is 32 32-bit words ([n, 32] int32 on the host)");
+    const char* fn = "moco_augment_crops_blur";
+    if (!norm || (dst_dtype != MOCO_F32 && dst_dtype != MOCO_BF16) ||
+        (n_crops > 0 && (!pixels || pixels_bytes == 0 || !crops || !dst || !crop_means || !aligned(crops, 8) ||
+                         !aligned(crop_means, 4) || !aligned(dst, dst_dtype == MOCO_F32 ? 4 : 2))))
+        return refuse(fn, MOCO_ERR_INVALID, "bad argument (null or misaligned pointer, empty pixel buffer, or "
+                      "dst_dtype=%d)", dst_dtype);
+    for (int k = 0; k < 6; ++k)
+        if (!isfinite(norm[k]) || (k >= 3 && norm[k] == 0.f))
+            return refuse(fn, MOCO_ERR_INVALID, "norm must be finite mean[3], std[3] with std != 0");
+    if (!augment_blur_shape_ok(n_crops, out_h, out_w, ksize))
+        return refuse(fn, MOCO_ERR_INVALID, "needs n_crops in [0, 65535], out_h, out_w in [1, 512] and an odd ksize in "
+                      "[3, 31] with ksize / 2 < min(out_h, out_w) (n_crops=%d out_h=%d out_w=%d ksize=%d)", n_crops,
+                      out_h, out_w, ksize);
+    return cuda_result(launch_augment_blur(pixels, pixels_bytes, crops, n_crops, out_h, out_w, ksize, norm, dst,
+                                           dst_dtype, crop_means, static_cast<cudaStream_t>(stream_)),
+                       "augment kernels");
+}
+
 int moco_resize_center_crops(const void* pixels, size_t pixels_bytes, const moco_resize_window* windows, int n,
                              int out_h, int out_w, const float* norm, void* dst, int dst_dtype, void* stream_) {
     g_err[0] = 0;

@@ -217,6 +217,10 @@ bool augment_shape_ok(int n_crops, int out_h, int out_w);
 cudaError_t launch_augment(const void* pixels, size_t pixels_bytes, const moco_aug_crop* crops, int n_crops, int out_h,
                            int out_w, const float norm[6], void* dst, int dst_dtype, float* crop_means,
                            cudaStream_t stream);
+bool augment_blur_shape_ok(int n_crops, int out_h, int out_w, int ksize);
+cudaError_t launch_augment_blur(const void* pixels, size_t pixels_bytes, const moco_aug_crop_blur* crops, int n_crops,
+                                int out_h, int out_w, int ksize, const float norm[6], void* dst, int dst_dtype,
+                                float* crop_means, cudaStream_t stream);
 cudaError_t launch_resize_windows(const void* pixels, size_t pixels_bytes, const moco_resize_window* windows, int n,
                                   int out_h, int out_w, const float norm[6], void* dst, int dst_dtype,
                                   cudaStream_t stream);

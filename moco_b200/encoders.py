@@ -99,9 +99,13 @@ class MoCoResNet(nn.Module):
     ``forward(x, layer)`` exits early as the reference's ``ResNet.forward(x, layer)`` (resnet.py:152-180) does, which
     its linear evaluation uses: layer <= 0 the input, 1 the stem's max-pool output, 2..5 the output of stage 1..4, 6
     the pooled and flattened features, 7 (default) the fc output, L2-normalised unless ``l2norm`` is off.
-    ``freeze()`` prepares the model for that evaluation (see its docstring)."""
+    ``freeze()`` prepares the model for that evaluation (see its docstring).
 
-    def __init__(self, block, depths, low_dim=128, width=1):
+    ``mlp=True`` gives MoCo v2's projection head: ``fc`` is Linear(C, C) -> ReLU -> Linear(C, low_dim), state-dict
+    keys ``fc.0.*`` and ``fc.2.*`` as in MoCo v2's checkpoints; the default is the bare Linear.  ``feat_dim`` (C) and
+    ``low_dim`` are the widths of layers 6 and 7 either way."""
+
+    def __init__(self, block, depths, low_dim=128, width=1, mlp=False):
         super().__init__()
         base = int(64 * width)
         # index 2 was the separate ReLU; kept as a placeholder so that the state_dict keys do not move
@@ -115,7 +119,11 @@ class MoCoResNet(nn.Module):
                 cin = planes * block.expansion
         self.layers = nn.Sequential(*layers)
         self.depths = list(depths)       # stage boundaries for forward(x, layer)
-        self.fc = nn.Linear(cin, low_dim)
+        self.feat_dim, self.low_dim = cin, low_dim
+        if mlp:
+            self.fc = nn.Sequential(nn.Linear(cin, cin), nn.ReLU(inplace=True), nn.Linear(cin, low_dim))
+        else:
+            self.fc = nn.Linear(cin, low_dim)
         # l2norm=False: return the raw fc output -- the contrast head then normalises inside its kernels
         # (MemoryMoCo.forward_loss(..., normalize=True), SURVEY.md 8 f2)
         self.l2norm = True
@@ -187,16 +195,30 @@ class MoCoResNet(nn.Module):
             return x
         return x / x.pow(2).sum(1, keepdim=True).sqrt()       # Normalize(power=2), resnet.py:30-33
 
-def resnet18(low_dim=128, width=1):
-    return MoCoResNet(_Basic, [2, 2, 2, 2], low_dim, width)
+def resnet18(low_dim=128, width=1, mlp=False):
+    return MoCoResNet(_Basic, [2, 2, 2, 2], low_dim, width, mlp)
 
 
-def resnet34(low_dim=128, width=1):
-    return MoCoResNet(_Basic, [3, 4, 6, 3], low_dim, width)
+def resnet34(low_dim=128, width=1, mlp=False):
+    return MoCoResNet(_Basic, [3, 4, 6, 3], low_dim, width, mlp)
 
 
-def resnet50(low_dim=128, width=1):
-    return MoCoResNet(_Bottleneck, [3, 4, 6, 3], low_dim, width)
+def resnet50(low_dim=128, width=1, mlp=False):
+    return MoCoResNet(_Bottleneck, [3, 4, 6, 3], low_dim, width, mlp)
+
+
+def has_mlp_head(sd) -> bool:
+    """Whether an encoder state_dict (either key naming, ``module.`` prefix optional) carries MoCo v2's MLP head."""
+    return any(k.removeprefix("module.").startswith("fc.0.") for k in sd)
+
+
+def encoder_from_state_dict(sd, arch="resnet50", width=1, low_dim=128):
+    """The ``arch`` encoder with the head ``sd`` carries (the MLP head or the bare Linear), ``sd`` loaded into it:
+    every driver that builds an encoder for a checkpoint goes through here."""
+    sd = from_reference_state_dict(sd)
+    model = {"resnet18": resnet18, "resnet34": resnet34, "resnet50": resnet50}[arch](low_dim, width, has_mlp_head(sd))
+    model.load_state_dict(sd)
+    return model
 
 
 # ---- checkpoints in the reference's naming ------------------------------------------------------------------------

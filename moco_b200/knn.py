@@ -152,7 +152,7 @@ def build_bank(model, loader, layer: int = 7, device=None) -> tuple[torch.Tensor
         x = A.resize_center_crops(b, dtype=torch.bfloat16, device=device)
         feats.append(_features(model, x, layer).bfloat16())
         labs.append(b[2].to(device, torch.int32))
-    dim = model.fc.out_features if layer == 7 else model.fc.in_features   # also for a rank with no samples
+    dim = model.low_dim if layer == 7 else model.feat_dim                 # also for a rank with no samples
     f = torch.cat(feats) if feats else torch.empty(0, dim, dtype=torch.bfloat16, device=device)
     lab = torch.cat(labs) if labs else torch.empty(0, dtype=torch.int32, device=device)
     world = dist.get_world_size() if dist.is_available() and dist.is_initialized() else 1
